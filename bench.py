@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- particle-steps/s of the particle/terrain hot path on B200 (BASELINE.json metric).
+"""bench.py -- particle-steps/s of the particle/terrain hot path on H100 (BASELINE.json metric).
 
 Workload (config 3 of BASELINE.json, the one the metric is quoted on that fits one GPU):
   4096^2 map, rockgravelpebblessand preset, SEED 42, per step (= one frame, SoilMachine.cpp:287-320
@@ -7,7 +7,7 @@ Workload (config 3 of BASELINE.json, the one the metric is quoted on that fits o
   WindParticles run to completion, then the frequency update.  particle-step = one move() followed by
   one interact() of one particle.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config 3|4|5]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config 3|4|5] [--dump-outputs DIR]
 
 * value   : whole-job particle-steps/s, spawn lists already resident in HBM, timed with CUDA events on the
             stream the kernels run on (max over ranks).
@@ -26,7 +26,12 @@ Workload (config 3 of BASELINE.json, the one the metric is quoted on that fits o
             genuinely HBM-bound full-grid kernels (mesh, frequency update, seep classification) with their bytes.
 * cpu_baseline / --impl reference: the reference's own CPU loop (oracle/_ref, the reference headers compiled
             verbatim) on a bounded sample of the same workload with the same water:wind mix, on the box's host
-            cores (1 thread: the reference is single-threaded and keeps its state in globals).
+            cores (1 thread: the reference is single-threaded and keeps its state in globals).  Left out (with
+            a note) where oracle/_ref has not been built.
+* --dump-outputs DIR: after the timed steps, what the last timed step left for a caller, as DIR/<name>.npy
+            (float32 / float64): the per-step counters of the timed steps, the column checksum, and a fixed
+            seeded sample of cells from the height field and the three frequency maps.  At N > 1 every rank
+            writes its own strip's set, named <name>_rank<r>.npy.
 N > 1: the SAME map is sharded into N x-strips, one rank (GPU) per strip; halo records, bins and hand-off words
 of the neighbouring strips are read and written over NVLink peer memory (CUDA IPC) by the sweep kernel itself,
 neighbouring strips synchronise every sweep, all strips every 8th, and particles that leave a strip are handed
@@ -64,7 +69,7 @@ def hbm_peak():
         with open(p) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md)"
+        return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3), not measured"
 
 
 class ClockSampler:
@@ -137,6 +142,35 @@ def checksum_sum(local, device=None):
     t = torch.tensor([v - (1 << 64) if v >= (1 << 63) else v], dtype=torch.int64, device=device)
     dist.all_reduce(t, op=dist.ReduceOp.SUM)
     return int(t.item()) & M64
+
+
+DUMP_SAMPLE = 1 << 20          # cells of each full-grid output written by --dump-outputs (fixed seeded sample)
+DUMP_SEED = 12345
+STAT_FIELDS = ("steps", "sweeps", "exit_oob", "exit_evap", "exit_stall", "pool_drops", "alive")
+
+
+def dump_outputs(d, ctx, counters, suffix=""):
+    """What the last timed step left for a caller of the path: the per-step counters of every timed step
+    (water then wind, STAT_FIELDS each), the column checksum of this context's columns as two 32-bit halves, and
+    the same seeded sample of cells (x, y) of this context's strip from the height field and from the three
+    frequency maps.  Heights are indexed (x - x0) * dimy + y over the strip, frequency maps y * dimx + x over the
+    whole map (include/soilmachine_b200.h), so each array is indexed in its own layout."""
+    import numpy as np
+    os.makedirs(d, exist_ok=True)
+    h = ctx.heights().reshape(-1)
+    idx = np.arange(h.size)
+    if h.size > DUMP_SAMPLE:
+        idx = np.sort(np.random.default_rng(DUMP_SEED).choice(h.size, size=DUMP_SAMPLE, replace=False))
+    x, y = ctx.x0 + idx // ctx.dimy, idx % ctx.dimy
+    cs = ctx.checksum()
+    out = {"sample_x": x.astype(np.float64), "sample_y": y.astype(np.float64), "heights": h[idx],
+           "column_checksum_hi_lo": np.array([cs >> 32, cs & 0xFFFFFFFF], np.float64),
+           "step_counters": np.array(counters, np.float64)}
+    fidx = y * ctx.dimx + x
+    for k, v in ctx.frequency().items():
+        out[k] = v[fidx]
+    for name, a in out.items():
+        np.save(os.path.join(d, name + suffix + ".npy"), a)
 
 
 def cpu_arm(W, steps, warmup):
@@ -284,6 +318,8 @@ def main():
     ap.add_argument("--particles", type=int, default=0, help="debug: override particles per kind")
     ap.add_argument("--no-cpu", action="store_true", help="skip the cpu_baseline leg")
     ap.add_argument("--no-extra", action="store_true", help="skip configs 4/5 and the full-grid kernels")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last one computed to DIR/<name>.npy")
     args = ap.parse_args()
 
     rank = int(os.environ.get("RANK", "0"))
@@ -368,18 +404,24 @@ def main():
     steps_w = steps_d = 0
     ms_w = ms_d = 0.0
     sweeps_w = sweeps_d = 0
+    counters = []
+    none = [0] * len(STAT_FIELDS)
     ctx.timer_start()
     t0 = time.perf_counter()
     for k in range(K):
+        cw = cd = none
         if dev[k][0] is not None:
             ctx.water_run_device(dev[k][0], W["nwater"])
             sw = ctx.last_stats()
             steps_w += sw.steps; ms_w += sw.device_ms; sweeps_w += sw.sweeps
+            cw = [getattr(sw, f) for f in STAT_FIELDS]
         if dev[k][1] is not None:
             ctx.wind_run_device(dev[k][1], W["nwind"])
             sd = ctx.last_stats()
             steps_d += sd.steps; ms_d += sd.device_ms; sweeps_d += sd.sweeps
+            cd = [getattr(sd, f) for f in STAT_FIELDS]
         ctx.frequency_update()
+        counters.append(cw + cd)
     ev_ms = ctx.timer_stop()
     barrier()
     wall_ms = (time.perf_counter() - t0) * 1e3
@@ -390,6 +432,8 @@ def main():
             ctx.device_free(a)
         if b is not None:
             ctx.device_free(b)
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, ctx, counters, "" if world == 1 else "_rank%d" % rank)
 
     # ---- e2e: host buffers through the public C ABI calls ----
     barrier()
@@ -449,14 +493,8 @@ def main():
     kern.sort(key=lambda x: -x[2])
     kname, ksteps, kms, kbytes, ksweeps = kern[0]
     achieved = (ksteps * kbytes / K) / (kms / K * 1e-3) / 1e9 if kms > 0 else 0.0
-    traffic = None
-    try:
-        with open(os.path.join(ROOT, "profiles", "traffic.json")) as f:
-            traffic = json.load(f).get(kname)
-    except Exception:
-        pass
     roofline = {"bound": "latency", "kernel": kname, "achieved": achieved, "peak": peak, "unit": "GB/s",
-                "frac": achieved / peak, "traffic": traffic, "peak_source": peak_src,
+                "frac": achieved / peak, "peak_source": peak_src,
                 "algorithmic_bytes_per_launch": ksteps * kbytes / K, "launch_ms": kms / K,
                 "share_of_step": kms / max(ms_w + ms_d, 1e-9),
                 "note": "dependency/latency-bound path (%d dependent sweeps per launch, ~%d B touched per particle-step): "
@@ -506,7 +544,10 @@ def main():
     if extra:
         line["extra"] = extra
 
-    if rank == 0 and world == 1 and not args.no_cpu:
+    from oracle import refapi
+    if rank == 0 and world == 1 and not args.no_cpu and not refapi.available():
+        line["cpu_baseline"] = {"skipped": "oracle/_ref not built (make -C oracle ref needs the reference sources)"}
+    elif rank == 0 and world == 1 and not args.no_cpu:
         _, info, _ = cpu_arm(W, 1, 0)
         # like for like: the reference's time for the particle-steps the GPU frame executed, per kind
         rw, rd = info["water_steps_per_s"], info["wind_steps_per_s"]

@@ -1,4 +1,4 @@
-/* soilmachine_b200 -- C ABI of the B200-native particle/terrain hot path.
+/* soilmachine_b200 -- C ABI of the H100-native particle/terrain hot path.
  *
  * The reference (weigert/SoilMachine) has no plugin or FFI layer: its frame loop
  * (SoilMachine.cpp:283-329) calls WaterParticle/WindParticle::move/interact

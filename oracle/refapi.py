@@ -9,6 +9,7 @@ import numpy as np
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "_ref", "libsmref.so")
 SOIL_DIR = os.path.join(HERE, "_ref", "soil")
+GOLDEN_SOIL_DIR = os.path.join(os.path.dirname(HERE), "tests", "golden", "soil")
 
 SOIL_DTYPE = np.dtype([
     ("name", "S32"),
@@ -37,10 +38,10 @@ def available():
 
 def soil_path(name):
     """Preset .soil file: the run-time copy under oracle/_ref/soil (made by `make -C oracle ref`),
-    else the reference tree when it is mounted."""
+    else the copy stored with the test fixtures (tests/golden/soil)."""
     if not name.endswith(".soil"):
         name += ".soil"
-    for d in (SOIL_DIR, "/root/reference/soil"):
+    for d in (SOIL_DIR, GOLDEN_SOIL_DIR):
         p = os.path.join(d, name)
         if os.path.exists(p):
             return p

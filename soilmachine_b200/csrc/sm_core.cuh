@@ -1,7 +1,7 @@
 // sm_core.cuh -- column operations and particle-step arithmetic of the hot path.
 //
 // Everything here is written against an "accessor" A that hands out mutable top-of-column
-// records, so the same arithmetic runs (a) inside the sm_100a sweep kernels on records staged in
+// records, so the same arithmetic runs (a) inside the sm_90a sweep kernels on records staged in
 // shared memory / read through L2, and (b) on the host inside the facade's single-cell calls.
 // The arithmetic is a type-exact transcription of the reference expressions: every float/double
 // promotion, association order and narrowing is kept, FMA contraction must be OFF

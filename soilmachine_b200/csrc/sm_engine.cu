@@ -1,4 +1,4 @@
-// sm_engine.cu -- sm_100a kernels and the C ABI of include/soilmachine_b200.h.
+// sm_engine.cu -- sm_90a kernels and the C ABI of include/soilmachine_b200.h.
 //
 // Hot path = k_run<KIND>: ONE persistent, co-resident kernel per particle batch.  Every sweep each
 // live particle executes move()+interact() (sm_core.cuh) exactly once; particles whose conflict
@@ -57,8 +57,8 @@ __device__ __forceinline__ int particle_reach(const WindP& p) {
 #endif
 #define SM_SWEEPS_NONE 0x40000000   // internal: run the prologue only
 #ifndef SM_DEFAULT_EXACT
-#define SM_DEFAULT_EXACT 1             // warp kernel: exact footprints for water batches (bit 0; measured -43 % on the
-                                       // water batch of config 3, -51 % on config 4, profiles/r02_exp12_exact_rounds.log), bit 1 = wind (-1 %)
+#define SM_DEFAULT_EXACT 1             // warp kernel: exact footprints for water batches (bit 0: shorter dependency
+                                       // chains in dense water clusters), bit 1 = wind
 #endif
 #ifndef SM_DEFAULT_COOP
 #define SM_DEFAULT_COOP true           // k_sweep (warp per particle); SM_KERNEL=thread selects the round-1 kernels
@@ -2066,8 +2066,8 @@ static bool hydro_warp() {
   const char* e = getenv("SM_HYDRO");
   if (e && strcmp(e, "warp") == 0) return true;
   if (e && strcmp(e, "thread") == 0) return false;
-  return false;     // measured (profiles/r02_exp2_timing.log): without a record cache the warp executor's seep pass is
-                    // 2-4x slower than the one-thread executor with its shared-memory cache; flood 0.7-1.5x
+  return false;     // without a record cache the warp executor's seep pass does not keep up with the one-thread
+                    // executor and its shared-memory cache
 }
 static int hydro_ready(sm_context* ctx) {
   if (ctx->nsoils < 1) return fail(ctx, SM_ERR_INVALID, "soil table not set");

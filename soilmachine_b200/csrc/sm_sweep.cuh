@@ -286,8 +286,8 @@ __device__ __forceinline__ unsigned int grid_barrier_x(const DevCtx& c, unsigned
 // The conservative rule orders two steps whenever their boxes (ipos +- R, R = 3 water, 3..5 wind) overlap, but a
 // water step really touches F = plus(ipos) U 3x3(npos) - about 14 of the 49 cells - and a wind step
 // plus(ipos) U 5x5(ipos) U 5x5(npos) (cascades around both cells with one nested re-cascade) out of up to 121; npos
-// is only known after move().  The per-sweep statistics (profiles/r02_sweepstat.log) show what that costs: in every
-// wind sweep some particle waits ~17 us for a chain of 2-3 boxes that overlap while the footprints do not.  With EXACT a
+// is only known after move(), so under boxes a particle can wait for a chain of 2-3 boxes that overlap while the
+// footprints do not.  With EXACT a
 // particle publishes three words per sweep: mv (= npos, right after move(); it only lets others SKIP a wait, so it
 // needs no fence), fin (its map writes are complete; release) and done (published in own-bin index order, which
 // keeps "X done => every lower index in X's bin done" and with it the crowded fallback sound).  A lower-index
@@ -614,7 +614,7 @@ __global__ void __launch_bounds__(SM_SW_WARPS * 32, SM_SW_MINBLOCKS) k_sweep(Dev
       bool exact_now = false;
       if constexpr (EXACT) {
         // (also for a particle with nothing in range: its mv word is what lets the particles behind it skip waits -
-        // sending those down the conservative path cost 15-20 %, profiles/r02_exp13_timing.log)
+        // sending those down the conservative path makes the particles behind it wait longer)
         exact_now = ws.cnt <= SM_SW_NEARX && !(MULTI && ws.remote);
         if (exact_now) r = sweep_exact<KIND, MULTI, BUDGET>(c, ws, w, s_soils, tag, pid, ix, iy, myR, p, edge);
       }
@@ -717,7 +717,7 @@ __global__ void __launch_bounds__(SM_SW_WARPS * 32, SM_SW_MINBLOCKS) k_sweep(Dev
 #if SM_PREFETCH
       // next sweep's records towards L2 while this sweep finishes: the 3x3 blocks around the next ipos and around
       // the position the current speed predicts after it (a wind particle covers fresh terrain every sweep; the
-      // map is 4x the L2)
+      // config-3 map is ten times the H100's 50 MB L2)
       if (r == SM_ALIVE && lane < 18) {
         const int ox = lane < 9 ? jx : (int)roundf(p.px + p.sx);
         const int oy = lane < 9 ? jy : (int)roundf(p.py + next_dy(p));

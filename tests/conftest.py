@@ -9,18 +9,15 @@ for p in (ROOT, os.path.join(ROOT, "tests")):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
 
 
 def _ensure_built():
-    """A fresh clone has no binaries (they are git-ignored): build what is missing and can be built here."""
+    """A fresh clone has no binaries (they are git-ignored): build the library if it is missing."""
     import subprocess
     lib = os.path.join(ROOT, "soilmachine_b200", "lib", "libsoilmachine_b200.so")
     if not os.path.exists(lib):
         subprocess.check_call(["bash", os.path.join(ROOT, "build.sh")])
-    ref = os.path.join(ROOT, "oracle", "_ref", "libsmref.so")
-    if not os.path.exists(ref) and os.path.isdir("/root/reference/source"):
-        subprocess.check_call(["make", "-C", os.path.join(ROOT, "oracle"), "ref"], stdout=subprocess.DEVNULL)
 
 
 _ensure_built()

@@ -1,6 +1,6 @@
 """Generates tests/golden/*.npz from the reference's own code (oracle/_ref/libsmref.so).
 
-Run where /root/reference is mounted (after `make -C oracle ref`):  python tests/golden/make_golden.py
+Run where the reference has been built (`make -C oracle ref`):  python tests/golden/make_golden.py
 The reference has no tests or golden vectors of its own (SURVEY.md section 4); these are outputs of the
 reference headers compiled verbatim, so every consumer (oracle port, product host build, CUDA path)
 is pinned to the same bits.
@@ -110,7 +110,26 @@ def hydro_case(soil, dim, seed, n, frames, name):
     print(name, "floods", floods, "air sections", int((c["type"] == 0).sum()), "saturated", int((c["saturation"] > 0).sum()))
 
 
+def loader_case():
+    """What the reference's loadsoil() makes of every preset file in tests/golden/soil (soil table, layer
+    table, world scale), and one spawn list drawn the way the particle constructors draw it."""
+    import glob
+    out = {}
+    for path in sorted(glob.glob(os.path.join(HERE, "soil", "*.soil"))):
+        name = os.path.basename(path)[:-5]
+        r = refapi.get().init(path, seed=0, dimx=8, dimy=8, poolsize=1000)
+        out[name + "/soils"], out[name + "/layers"] = r.soils(), r.layers()
+        out[name + "/scale"] = np.int64(r.scale)
+    r = refapi.get().init("default", seed=5, dimx=100, dimy=70)
+    out["spawn_default_100x70_seed5"] = r.spawn_list(64, seed=5)
+    np.savez_compressed(os.path.join(HERE, "ref_loader.npz"), **out)
+    print("ref_loader", len(out), "arrays")
+
+
 if __name__ == "__main__":
+    if len(sys.argv) > 1 and sys.argv[1] == "loader":
+        loader_case()
+        sys.exit(0)
     if len(sys.argv) > 1 and sys.argv[1] == "hydro":
         hydro_case("default", 48, 42, 400, 3, "hydro_default_48")
         hydro_case("bigbutte", 40, 3, 500, 3, "hydro_bigbutte_40")

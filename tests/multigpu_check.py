@@ -3,7 +3,7 @@ must be bit-identical to the same frames on one unsharded context.  Rank 0 runs 
 compares heights, every column section (checksum), frequency maps and the counters; prints one line and exits
 non-zero on any difference.
 
-  N GPUs (gpurun --gpus N), one rank per GPU, NCCL for the plumbing:
+  N GPUs, one rank per GPU, NCCL for the plumbing:
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P \
         tests/multigpu_check.py [dim] [particles] [soil]
   ONE GPU, N processes sharing it (what the 1-GPU test tier runs, tests/test_gpu_parity.py): SM_ONE_GPU=1 in the

@@ -33,32 +33,34 @@ def test_no_cpu_fallback():
     assert e.value.code == smb.capi.SM_ERR_NOGPU
 
 
-def test_presets_match_reference_loader(ref):
+def test_presets_match_reference_loader():
+    """The JSON presets against what the reference's loadsoil() made of each preset file (tests/golden)."""
+    import _golden
     from soilmachine_b200 import presets
+    g = _golden.load("ref_loader")
     names = presets.names()
     assert "rockgravelpebblessand" in names and len(names) == 11
     for name in names:
-        ref.init(name, seed=0, dimx=8, dimy=8, poolsize=1000)
         pre = presets.load(name)
-        rs, rl = ref.soils(), ref.layers()
+        rs, rl = g[name + "/soils"], g[name + "/layers"]
         assert len(rs) == len(pre["soils"]) and len(rl) == len(pre["layers"])
         for k in pre["soils"].dtype.names:
             assert np.array_equal(rs[k], pre["soils"][k]), (name, k)
         for k in pre["layers"].dtype.names:
             assert np.array_equal(rl[k], pre["layers"][k]), (name, k)
-        assert ref.scale == pre["world"]["scale"]
+        assert int(g[name + "/scale"]) == pre["world"]["scale"]
 
 
-def test_spawn_lists_match_reference_ctor_draws(ref):
+def test_spawn_lists_match_reference_ctor_draws():
+    import _golden
     from soilmachine_b200 import host
-    ref.init("default", seed=5, dimx=100, dimy=70)
-    a = ref.spawn_list(64, seed=5)
+    a = _golden.load("ref_loader")["spawn_default_100x70_seed5"]
     host.srand(5)
     b = host.spawn_list(64, 100, 70)
     assert np.array_equal(a, b)
 
 
-def test_bench_reference_arm_runs():
+def test_bench_reference_arm_runs(ref):
     out = subprocess.run([sys.executable, os.path.join(ROOT, "bench.py"), "--impl", "reference", "--dim", "96",
                           "--particles", "200", "--steps", "1", "--warmup", "0"],
                          capture_output=True, text=True, timeout=300, cwd=ROOT)
@@ -94,19 +96,19 @@ def test_cpp_facade_compiles_and_links():
         assert out.returncode == 77 and "no CUDA device" in out.stdout
 
 
-def test_soil_file_parser_matches_reference_loader(ref):
-    """include/soilmachine/soilfile.hpp (restatement of loadsoil, io.h:7-230, quirks included) against the
-    reference loader itself on every preset file, and against the committed JSON presets."""
+def test_soil_file_parser_matches_reference_loader():
+    """include/soilmachine/soilfile.hpp (restatement of loadsoil, io.h:7-230, quirks included) against what the
+    reference loader made of every preset file (tests/golden), and against the committed JSON presets."""
     import glob
-    from oracle import refapi
+    import _golden
     from soilmachine_b200 import capi, presets
-    files = sorted(glob.glob(os.path.join(os.path.dirname(refapi.soil_path("default")), "*.soil")))
+    g = _golden.load("ref_loader")
+    files = sorted(glob.glob(os.path.join(_golden.GOLDEN, "soil", "*.soil")))
     assert len(files) == 11
     for path in files:
         name = os.path.basename(path)[:-5]
         got = capi.parse_soil_file(path)
-        ref.init(path, seed=0, dimx=8, dimy=8, poolsize=1000)
-        rs, rl = ref.soils(), ref.layers()
+        rs, rl = g[name + "/soils"], g[name + "/layers"]
         assert got["soil_names"] == [s.decode() for s in rs["name"]], name
         for k in got["soils"].dtype.names:
             assert np.array_equal(got["soils"][k], rs[k]), (name, k)

@@ -132,18 +132,19 @@ def test_initialize_matches_reference_terrain(ref, soil, dim, seed):
         _same(c1[k], c2[k], "init columns." + k)
 
 
-def test_presets_match_reference_loader(ref):
+def test_presets_match_reference_loader():
+    import _golden
     from soilmachine_b200 import presets
+    g = _golden.load("ref_loader")
     for name in presets.names():
-        ref.init(name, seed=0, dimx=8, dimy=8, poolsize=1000)
         pre = presets.load(name)
-        rs, rl = ref.soils(), ref.layers()
+        rs, rl = g[name + "/soils"], g[name + "/layers"]
         assert len(rs) == len(pre["soils"]) and len(rl) == len(pre["layers"])
         for k in pre["soils"].dtype.names:
             _same(rs[k], pre["soils"][k], name + ".soils." + k)
         for k in pre["layers"].dtype.names:
             _same(rl[k], pre["layers"][k], name + ".layers." + k)
-        assert ref.scale == pre["world"]["scale"]
+        assert int(g[name + "/scale"]) == pre["world"]["scale"]
 
 
 def test_smoke_entry():

@@ -187,9 +187,12 @@ def test_gpu_wind_particles_follow_the_lattice_field(ref):
     po.set_columns(cols)
     po.set_wind_field(v4, dims)
     xy = ref.spawn_list(n, seed=9)
-    r, g = po.wind_run(xy), ctx.wind_run(xy)
+    # some particles never leave this field (they circle in the lee of the terrain), so the batch is cut after a
+    # fixed number of sweeps on both sides; the particles still alive then are compared like the others
+    sweeps = 3000
+    r, g = po.wind_run(xy, max_sweeps=sweeps), ctx.wind_run(xy, max_sweeps=sweeps)
     po.set_wind_field(None)
-    assert (g.steps, g.exit_oob) == (r.steps, r.exit_oob) and g.steps > 0
+    assert (g.steps, g.sweeps, g.exit_oob) == (r.steps, r.sweeps, r.exit_oob) and g.steps > 0
     a, b = ctx.wind_state(), po.wind_state()
     for k in b:
         assert np.array_equal(np.ascontiguousarray(a[k]).view(np.uint8), np.ascontiguousarray(b[k]).view(np.uint8)), k
