@@ -1908,7 +1908,8 @@ static int launch_run(sm_context* ctx, int kind, int n, const float* d_spawn, in
     if (e && strcmp(e, "warp") == 0) use_coop = true;
   }
   if (use_coop) {
-    const int cthreads = SM_SW_WARPS * 32;
+    const int sw_warps = kind == KIND_WIND ? SwShape<KIND_WIND>::WARPS : SwShape<KIND_WATER>::WARPS;
+    const int cthreads = sw_warps * 32;
     int occ = 0;
     const bool budget = ctx->d.bud != nullptr;
     // SM_EXACT: bit mask of the kinds that use exact footprints (sweep_exact): 1 = water, 2 = wind
@@ -1933,7 +1934,7 @@ static int launch_run(sm_context* ctx, int kind, int n, const float* d_spawn, in
     if (occ < 1) return fail(ctx, SM_ERR_CUDA, "sweep kernel does not fit an SM");
     // contexts that share the device must all be resident at once (they meet in the cross-rank barrier)
     const long long maxblocks = std::max<long long>(1, (long long)ctx->num_sms * occ / ctx->share);
-    const long long want = ((long long)std::max(n, 1) + SM_SW_WARPS - 1) / SM_SW_WARPS;
+    const long long want = ((long long)std::max(n, 1) + sw_warps - 1) / sw_warps;
     const int cblocks = (int)std::max<long long>(1, std::min(maxblocks, want));
     DevCtx dd = ctx->d;
     int ms = max_sweeps;

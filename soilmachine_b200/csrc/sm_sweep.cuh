@@ -14,12 +14,13 @@
 #pragma once
 #include "sm_coop.cuh"
 
-#ifndef SM_SW_WARPS
-#define SM_SW_WARPS 8        // warps (= particles in flight) per block
-#endif
-#ifndef SM_SW_MINBLOCKS
-#define SM_SW_MINBLOCKS 3    // resident blocks per SM the kernel is compiled for (register cap)
-#endif
+// Block shape by kind: warps (= particles in flight) per block and resident blocks per SM the kernel is compiled for
+// (which sets the register cap).  Wind: 2 x 10 warps, a 96-register cap (65536 / 640 threads) that halves the spills
+// of the latency-bound wind step; water: 3 x 8 at 80 registers, where a large batch needs every warp (DESIGN.md K1/K2).
+template <int KIND> struct SwShape {
+  static constexpr int WARPS = (KIND == KIND_WIND) ? 10 : 8;
+  static constexpr int MINBLOCKS = (KIND == KIND_WIND) ? 2 : 3;
+};
 #define SM_SW_NEAR 31        // in-range lower-index particles tracked exactly (one polling lane each)
 #define SM_SW_NEARX 128      // ... by the exact schedule, which polls them in rounds of 32 (dense clusters - water
                              // collecting in a pit - are where exact footprints pay most: scripts/chain_analysis.py)
@@ -453,12 +454,13 @@ __device__ __forceinline__ unsigned int live_total(const unsigned int* __restric
 }
 
 template <int KIND, bool MULTI, bool BUDGET, bool EXACT>
-__global__ void __launch_bounds__(SM_SW_WARPS * 32, SM_SW_MINBLOCKS) k_sweep(DevCtx c, int n, const float* __restrict__ spawn,
+__global__ void __launch_bounds__(SwShape<KIND>::WARPS * 32, SwShape<KIND>::MINBLOCKS) k_sweep(DevCtx c, int n, const float* __restrict__ spawn,
                                                                             int max_sweeps) {
   typedef typename PType<KIND>::T P;
+  constexpr int NWARPS = SwShape<KIND>::WARPS;
   __shared__ SoilDev s_soils[SM_MAX_SOILS];
-  __shared__ unsigned int s_alive, s_total, s_wsum[SM_SW_WARPS];
-  __shared__ WarpSmem s_w[SM_SW_WARPS];
+  __shared__ unsigned int s_alive, s_total, s_wsum[NWARPS];
+  __shared__ WarpSmem s_w[NWARPS];
   extern __shared__ unsigned int s_live[];          // [0, W): this sweep's live mask, [W, 2W): exclusive popcount prefix
   const int W = (n + 31) >> 5;
   unsigned int* const s_word = s_live;
@@ -474,8 +476,8 @@ __global__ void __launch_bounds__(SM_SW_WARPS * 32, SM_SW_MINBLOCKS) k_sweep(Dev
   const int gtid = blockIdx.x * blockDim.x + threadIdx.x;
   const int lane = threadIdx.x & 31;
   const int wib = threadIdx.x >> 5;
-  const int slot = blockIdx.x * SM_SW_WARPS + wib;
-  const int nslots = gridDim.x * SM_SW_WARPS;
+  const int slot = blockIdx.x * NWARPS + wib;
+  const int nslots = gridDim.x * NWARPS;
   WarpSmem& ws = s_w[wib];
   WarpDev w{lane};
 
@@ -546,7 +548,7 @@ __global__ void __launch_bounds__(SM_SW_WARPS * 32, SM_SW_MINBLOCKS) k_sweep(Dev
   for (;; s++) {
     const unsigned int tag = tag0 + (unsigned int)s;
     if (max_sweeps >= 0 && s >= max_sweeps) {
-      if (!MULTI) total_alive = live_total<SM_SW_WARPS>(c.lmask[tag % 3u], W, s_word, s_pref, s_wsum);
+      if (!MULTI) total_alive = live_total<NWARPS>(c.lmask[tag % 3u], W, s_word, s_pref, s_wsum);
       break;
     }
     // ---- who is alive, in index order ------------------------------------------------------------------------
@@ -556,7 +558,7 @@ __global__ void __launch_bounds__(SM_SW_WARPS * 32, SM_SW_MINBLOCKS) k_sweep(Dev
     // - ascending index within a warp (no wait can cycle), and every warp gets the same share whatever the pattern
     // of deaths is.  (With a fixed particle -> warp map the warp holding the most survivors set the pace of the
     // sweep: 5-6 of its 7 particles where the average is under 2.)
-    const unsigned int live = live_total<SM_SW_WARPS>(c.lmask[tag % 3u], W, s_word, s_pref, s_wsum);
+    const unsigned int live = live_total<NWARPS>(c.lmask[tag % 3u], W, s_word, s_pref, s_wsum);
     if (!MULTI) total_alive = live;
     if ((!MULTI || xglobal) && total_alive == 0) break;
     {   // the mask two sweeps ahead becomes the survivors' mask of the next sweep: clear it now
