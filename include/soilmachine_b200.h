@@ -87,7 +87,16 @@ int sm_sync(sm_context* ctx);
  * sm_initialize / sm_upload_columns / downloads work on the rank's own strip (cell order
  * (x - x0)*dimy + y) and sm_*_run_device must be called on EVERY rank (the kernels meet in a cross-rank
  * barrier every sweep); results are bit-identical to the unsharded run.  share = number of contexts
- * that run their kernels concurrently on this device. */
+ * that run their kernels concurrently on this device.
+ * Read-only views of the whole map also work on a sharded context: sm_mesh_update / sm_mesh_device_ptr /
+ * sm_export_* cover the rank's own strip (cell order (x - x0)*dimy + y, i.e. the slice [x0*dimy, x1*dimy) of the
+ * unsharded arrays); sm_cell_query / sm_height_bilinear / sm_cell_column take global coordinates of any cell, on any
+ * rank; sm_lbm_set_boundary(ctx, NULL) builds the boundary of the whole lattice from the whole map.  All of these
+ * read other ranks' strips, so before calling any of them every rank's earlier work on the map (a batch,
+ * sm_initialize, sm_upload_columns) must have completed: sm_sync on every rank, then a host barrier; and no rank may
+ * change its strip again until the other ranks' calls have returned (a batch is safe: its ranks meet in a barrier
+ * before any of them writes).  The pooling hydrology and the single-cell calls that change the map return
+ * SM_ERR_INVALID on a sharded context. */
 #define SM_PEER_ARRAYS 20
 #define SM_PEER_SLOTS 24
 typedef struct sm_peer_blob {
@@ -146,7 +155,7 @@ int sm_set_soil_colors(sm_context* ctx, const float* rgba, int32_t n);
 /* Layermap::update(Vertexpool&) (layermap.h:551-555 = update(ivec2,...) :475-549 for every cell): one
  * 44-byte Vertex {position[3], normal[3], color[4], index} per cell in cell order, sliced at the plane
  * SLICE (SoilMachine.cpp:12).  The vertices stay in device memory (sm_mesh_device_ptr, e.g. for GL
- * interop); host_vertices may be NULL or a buffer of cells*11 floats. */
+ * interop); host_vertices may be NULL or a buffer of cells*11 floats (cells of this rank's strip on a sharded map). */
 int sm_mesh_update(sm_context* ctx, int32_t slice, float* host_vertices);
 int sm_mesh_device_ptr(sm_context* ctx, void** dptr);
 /* exportheight / exportcolor (io.h:234-252): the values the reference writes to the PNGs, as floats:
@@ -243,7 +252,11 @@ int sm_seep(sm_context* ctx, sm_hydro_stats* stats);
  * floats, > 0 = obstacle); sm_lbm_step = n x (collide.cs + stream.cs) fused into one kernel per step
  * (lbmwind.h:170-187); sm_lbm_get: populations in upstream's layout F[cell*19 + q] with cell = (x*ny + y)*nz + z,
  * density, velocity (x, y, z, w); sm_lbm_advect = move.cs (tracer particles, n x (x, y, z, w), in place).
- * Arithmetic is defined by oracle/lbm_oracle.c (parity with the GLSL unpinned: no GL here, no reference vectors). */
+ * Arithmetic is defined by oracle/lbm_oracle.c (parity with the GLSL unpinned: no GL here, no reference vectors).
+ * Sharded map: the lattice is not sharded; every rank keeps a full, identical copy.  Every rank calls sm_lbm_create
+ * with the same dimensions, builds the same boundary (NULL: from the whole map, with the precondition of the
+ * sharded-map paragraph above) and steps the lattice the same number of times; sm_lbm_get returns the rank's full
+ * lattice, and sm_wind_use_lbm couples each rank's wind particles to its own copy. */
 int sm_lbm_create(sm_context* ctx, int32_t nx, int32_t ny, int32_t nz);
 int sm_lbm_set_boundary(sm_context* ctx, const float* boundary);
 int sm_lbm_init(sm_context* ctx);                        /* init.cs again, with the current boundary */

@@ -111,6 +111,64 @@ class VirtualShards:
     def wind_run(self, xy, max_sweeps=0):
         return self._run("wind", xy, max_sweeps)
 
+    # ---- read-only views of the whole map (meshing, export, queries, wind-field boundary) ----
+    # Each of these reads other ranks' strips, so every rank's earlier work must have completed first: sync() does
+    # that for contexts of this process.
+    def sync(self):
+        for c in self.ctx:
+            c.sync()
+
+    def set_soil_colors(self, rgba):
+        for c in self.ctx:
+            c.set_soil_colors(rgba)
+
+    def mesh_update(self, slice_):
+        """the full-map vertex array (cells, 11), cell order x*dimy + y: every rank meshes its own strip"""
+        self.sync()
+        return np.concatenate([c.mesh_update(slice_) for c in self.ctx], axis=0)
+
+    def export_height(self):
+        return np.concatenate([c.export_height() for c in self.ctx])
+
+    def export_color(self):
+        return np.concatenate([c.export_color() for c in self.ctx], axis=0)
+
+    def cell_query(self, x, y, rank=0):
+        """global coordinates, any cell of the map; `rank` is the context that issues the call"""
+        self.sync()
+        return self.ctx[rank].cell_query(x, y)
+
+    def height_bilinear(self, x, y, rank=0):
+        self.sync()
+        return self.ctx[rank].height_bilinear(x, y)
+
+    def cell_column(self, x, y, capacity=64, rank=0):
+        self.sync()
+        return self.ctx[rank].cell_column(x, y, capacity)
+
+    # ---- wind field: every rank keeps the whole lattice (identical on every rank) ----
+    def lbm_create(self, nx, ny, nz):
+        for c in self.ctx:
+            c.lbm_create(nx, ny, nz)
+
+    def lbm_set_boundary(self, boundary=None):
+        """None: from the terrain of the whole map, built by every rank"""
+        if boundary is None:
+            self.sync()
+        for c in self.ctx:
+            c.lbm_set_boundary(boundary)
+
+    def lbm_step(self, n=1):
+        """device milliseconds of each rank's steps"""
+        return [c.lbm_step(n) for c in self.ctx]
+
+    def wind_use_lbm(self, on=True):
+        for c in self.ctx:
+            c.wind_use_lbm(on)
+
+    def lbm_get(self, rank=0):
+        return self.ctx[rank].lbm_get()
+
 
 class DistShard:
     """This process's rank of a map sharded over torch.distributed ranks (one GPU each)."""
@@ -134,6 +192,58 @@ class DistShard:
         """launch this rank's sweep kernel (all ranks must call it), wait, return local stats"""
         (self.ctx.water_run_device if kind == "water" else self.ctx.wind_run_device)(d_xy, n, max_sweeps)
         return self.ctx.last_stats()
+
+    # ---- read-only views of the whole map ----
+    # The calls that read other ranks' strips first wait for this rank's work and then meet every other rank in a
+    # barrier, so all ranks must call them (each with its own arguments).
+    def _settle(self):
+        self.ctx.sync()
+        self.dist.barrier()
+
+    def set_soil_colors(self, rgba):
+        self.ctx.set_soil_colors(rgba)
+
+    def mesh_update(self, slice_):
+        """this rank's strip of the vertex array ((x1 - x0)*dimy, 11), cell order (x - x0)*dimy + y"""
+        self._settle()
+        return self.ctx.mesh_update(slice_)
+
+    def export_height(self):
+        return self.ctx.export_height()
+
+    def export_color(self):
+        return self.ctx.export_color()
+
+    def cell_query(self, x, y):
+        """global coordinates, any cell of the map"""
+        self._settle()
+        return self.ctx.cell_query(x, y)
+
+    def height_bilinear(self, x, y):
+        self._settle()
+        return self.ctx.height_bilinear(x, y)
+
+    def cell_column(self, x, y, capacity=64):
+        self._settle()
+        return self.ctx.cell_column(x, y, capacity)
+
+    # ---- wind field: every rank keeps the whole lattice; all ranks make the same calls ----
+    def lbm_create(self, nx, ny, nz):
+        self.ctx.lbm_create(nx, ny, nz)
+
+    def lbm_set_boundary(self, boundary=None):
+        if boundary is None:
+            self._settle()
+        self.ctx.lbm_set_boundary(boundary)
+
+    def lbm_step(self, n=1):
+        return self.ctx.lbm_step(n)
+
+    def wind_use_lbm(self, on=True):
+        self.ctx.wind_use_lbm(on)
+
+    def lbm_get(self):
+        return self.ctx.lbm_get()
 
     def close(self):
         self.dist.barrier()
