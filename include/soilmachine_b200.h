@@ -58,7 +58,8 @@ typedef struct sm_config {
   int32_t max_particles;    /* largest batch a *_run call will be given; 0 = 262144 */
   int32_t flags;            /* SM_FLAG_* */
 } sm_config;
-#define SM_FLAG_BUDGET 1      /* keep the per-particle mass budget (sm_last_budget); a few % slower */
+#define SM_FLAG_BUDGET 1      /* keep the per-particle mass budget (sm_last_budget) and the hydrology's
+                                 (sm_last_hydro_budget); a few % slower */
 
 /* Per-call counters (all accumulated over the call). */
 typedef struct sm_stats {
@@ -244,6 +245,30 @@ int sm_water_flood(sm_context* ctx, sm_hydro_stats* stats);
 /* WaterParticle::seep(map, vertexpool) (water.h:335-343): the per-frame pass over all cells in x-major
  * order, seep(cell) then the water-table cascade with spill 3. */
 int sm_seep(sm_context* ctx, sm_hydro_stats* stats);
+/* Mass budget of the last successful sm_water_flood or sm_seep call (contexts created with SM_FLAG_BUDGET; such a
+ * context runs both on the warp executor whatever SM_HYDRO says).  Same rules as sm_budget: each term is a change
+ * of column height (floor + top size) read right before and right after the column operation, accumulated in
+ * execution order, bit-identical to the oracle port's accumulators.  The terms are heights, not materials: a
+ * remove on an Air-topped column takes water first, so nested_eroded can include water.  The single-cell calls
+ * (sm_cell_seep, sm_cell_water_cascade) are not covered.
+ * Identity: change of (sum of all column heights) = flood_sediment + flood_cascade_net + flood_water - seeped
+ *           - to_particles + transfer_net + nested_deposited - nested_eroded + nested_cascade_net, to rounding.
+ * SM_ERR_INVALID without SM_FLAG_BUDGET or before the first hydrology call. */
+typedef struct sm_hydro_budget {
+  double flood_sediment;      /* height added by the floods' sediment add                        (water.h:133) */
+  double flood_cascade_net;   /* net height change of the floods' terrain cascade, as cascade_net (water.h:134) */
+  double flood_water;         /* height added by the floods' Air add                             (water.h:138) */
+  double seeped;              /* height of standing water removed by seep(cell), positive: inside the floods and
+                                 in the seep pass (water.h:318-319) */
+  double to_particles;        /* height removed when a whole water section leaves as a nested particle (water.h:248) */
+  double transfer_net;        /* partial water-table transfers: height lost + height gained (water.h:268-271) */
+  double nested_eroded;       /* sm_budget's eroded, deposited, cascade_net, discarded and clamped, summed over */
+  double nested_deposited;    /*   every step of every particle the water-table cascade spawned (water.h:252-253) */
+  double nested_cascade_net;
+  double nested_discarded;
+  double nested_clamped;
+} sm_hydro_budget;
+int sm_last_hydro_budget(sm_context* ctx, sm_hydro_budget* budget);
 
 /* ---- wind field: D3Q19 lattice Boltzmann, TRT collision (source/include/lbmwind/) ------------------------------
  * The reference runs this as OpenGL compute shaders and only draws it (WindParticle keeps a constant prevailing

@@ -36,7 +36,7 @@ SYMBOLS = [
     "sm_wind_sweeps", "sm_wind_state", "sm_launch_count", "sm_device_alloc", "sm_device_free",
     "sm_device_upload", "sm_timer_start", "sm_timer_stop", "sm_set_soil_colors", "sm_mesh_update",
     "sm_mesh_device_ptr", "sm_export_height", "sm_export_color", "sm_create_sharded", "sm_shard_range",
-    "sm_peer_export", "sm_peer_attach", "sm_parse_soil_file", "sm_water_flood", "sm_seep", "sm_last_budget", "sm_budget_particles", "sm_lbm_create", "sm_lbm_set_boundary", "sm_lbm_init",
+    "sm_peer_export", "sm_peer_attach", "sm_parse_soil_file", "sm_water_flood", "sm_seep", "sm_last_budget", "sm_budget_particles", "sm_last_hydro_budget", "sm_lbm_create", "sm_lbm_set_boundary", "sm_lbm_init",
     "sm_lbm_step", "sm_lbm_get", "sm_lbm_advect", "sm_wind_use_lbm",
 ]
 
@@ -68,6 +68,15 @@ class Budget(C.Structure):
     _fields_ = [("eroded", C.c_double), ("deposited", C.c_double), ("cascade_net", C.c_double),
                 ("discarded", C.c_double), ("clamped", C.c_double), ("wind_negative", C.c_double),
                 ("particles", C.c_int64)]
+
+    def asdict(self):
+        return {k: getattr(self, k) for k, _ in self._fields_}
+
+
+class HydroBudget(C.Structure):
+    _fields_ = [(k, C.c_double) for k in (
+        "flood_sediment", "flood_cascade_net", "flood_water", "seeped", "to_particles", "transfer_net",
+        "nested_eroded", "nested_deposited", "nested_cascade_net", "nested_discarded", "nested_clamped")]
 
     def asdict(self):
         return {k: getattr(self, k) for k, _ in self._fields_}
@@ -393,6 +402,13 @@ class Context:
         st = HydroStats()
         self._ck(self.lib.sm_seep(self.h, C.byref(st)))
         return st
+
+    def last_hydro_budget(self):
+        """mass budget of the last water_flood or seep call (context created with budget=True): a dict of the
+        eleven sm_hydro_budget terms (include/soilmachine_b200.h)"""
+        b = HydroBudget()
+        self._ck(self.lib.sm_last_hydro_budget(self.h, C.byref(b)))
+        return b.asdict()
 
     def water_begin(self, xy):
         xy = np.ascontiguousarray(xy, np.float32)

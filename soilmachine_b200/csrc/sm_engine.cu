@@ -1218,31 +1218,47 @@ __global__ void __launch_bounds__(32) k_hydro_seep(DevCtx c, ActiveMap am, Hydro
 // ---- the same two phases executed by one WARP (sm_hydro_coop.cuh): frames evaluated eight neighbours at a time,
 // nested particles on the cooperative step.  Records are accessed in place through L2 (a frame's nine records are
 // fetched by nine lanes at once, which is what the one-thread executor needs its shared-memory cache for).
-struct HydroBack : DevBack<false, false> {
+// BUDGET: the hydrology's mass budget (HydroScratchBudget::bud, sm_hydro_coop.cuh), for contexts created with SM_FLAG_BUDGET.
+template <bool BUDGET> struct HydroBack : DevBack<false, BUDGET> {
   static constexpr bool kHydroHooks = true;
   ActiveMap act;
   bool marking;
   __device__ __forceinline__ HydroBack(const DevCtx& ctx, const SoilDev* ss, const ActiveMap& am, bool mk)
-      : DevBack<false, false>(ctx, ss, 0u), act(am), marking(mk) {}
+      : DevBack<false, BUDGET>(ctx, ss, 0u), act(am), marking(mk) {}
   // single writer: only the lane that mutates columns calls these
   __device__ __forceinline__ void air_mark(Sec32* r, int x, int y) {
-    if (marking && r->type == SM_AIR) active_mark_block(act, x, y, c.dimx, c.dimy);
+    if (marking && r->type == SM_AIR) active_mark_block(act, x, y, this->c.dimx, this->c.dimy);
   }
   __device__ __forceinline__ void wet_mark(int x, int y) {
-    if (marking) active_set(act, (unsigned long long)x * c.dimy + y);
+    if (marking) active_set(act, (unsigned long long)x * this->c.dimy + y);
   }
 };
-__global__ void __launch_bounds__(32) k_hydro_flood_w(DevCtx c, int n, HydroCount* out) {
+// what a hydrology call hands back: its counters, and with BUDGET the eleven budget sums
+struct HydroTotals {
+  HydroCount hc;
+  double bud[SM_HYDRO_BUDGET_SLOTS];
+};
+template <bool BUDGET, class S> __device__ __forceinline__ void hydro_budget_zero(S& hx, int lane) {
+  if constexpr (BUDGET) if (lane == 0)
+    for (int k = 0; k < SM_HYDRO_BUDGET_SLOTS; k++) hx.bud[k] = 0.0;
+}
+template <bool BUDGET, class S> __device__ __forceinline__ void hydro_totals_out(HydroTotals* out, const HydroCount& hc, const S& hx) {
+  hydro_count_out(&out->hc, hc);
+  if constexpr (BUDGET)
+    for (int k = 0; k < SM_HYDRO_BUDGET_SLOTS; k++) out->bud[k] = hx.bud[k];
+}
+template <bool BUDGET> __global__ void __launch_bounds__(32) k_hydro_flood_w(DevCtx c, int n, HydroTotals* out) {
   __shared__ SoilDev s_soils[SM_MAX_SOILS];
   __shared__ CoopScratch sc;
-  __shared__ HydroScratch hx;
+  __shared__ typename HydroScratchOf<BUDGET>::type hx;
   const int lane = threadIdx.x;
   for (int i = lane; i < c.nsoils; i += 32) s_soils[i] = c.soils[i];
+  hydro_budget_zero<BUDGET>(hx, lane);
   __syncwarp();
   WarpDev w{lane};
   ActiveMap none{};
-  HydroBack back(c, s_soils, none, false);
-  CoopWin<HydroBack> a(back, &sc);
+  HydroBack<BUDGET> back(c, s_soils, none, false);
+  CoopWin<HydroBack<BUDGET> > a(back, &sc);
   HydroCount hc{};
   for (int base = 0; base < n; base += 32) {
     const int i = base + lane;
@@ -1262,25 +1278,26 @@ __global__ void __launch_bounds__(32) k_hydro_flood_w(DevCtx c, int n, HydroCoun
       __syncwarp();
     }
   }
-  if (lane == 0) hydro_count_out(out, hc);
+  if (lane == 0) hydro_totals_out<BUDGET>(out, hc, hx);
 }
-__global__ void __launch_bounds__(32) k_hydro_seep_w(DevCtx c, ActiveMap am, HydroCount* out) {
+template <bool BUDGET> __global__ void __launch_bounds__(32) k_hydro_seep_w(DevCtx c, ActiveMap am, HydroTotals* out) {
   __shared__ SoilDev s_soils[SM_MAX_SOILS];
   __shared__ CoopScratch sc;
-  __shared__ HydroScratch hx;
+  __shared__ typename HydroScratchOf<BUDGET>::type hx;
   const int lane = threadIdx.x;
   for (int i = lane; i < c.nsoils; i += 32) s_soils[i] = c.soils[i];
+  hydro_budget_zero<BUDGET>(hx, lane);
   __syncwarp();
   WarpDev w{lane};
-  HydroBack back(c, s_soils, am, true);
-  CoopWin<HydroBack> a(back, &sc);
+  HydroBack<BUDGET> back(c, s_soils, am, true);
+  CoopWin<HydroBack<BUDGET> > a(back, &sc);
   HydroCount hc{};
   const unsigned long long cells = am.ncells;
   for (unsigned long long cell = active_next(am, 0); cell < cells; cell = active_next(am, cell + 1)) {
     hydro_seep_visit_coop(w, a, &hx, (int)(cell / (unsigned long long)c.dimy), (int)(cell % (unsigned long long)c.dimy), hc);
     __syncwarp();
   }
-  if (lane == 0) hydro_count_out(out, hc);
+  if (lane == 0) hydro_totals_out<BUDGET>(out, hc, hx);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1309,7 +1326,9 @@ struct sm_context {
   bool mesh_valid = false;
   unsigned long long* d_act = nullptr;   // active-cell index of the seep pass (allocated on first use)
   unsigned long long act_words = 0;
-  HydroCount* d_hydro = nullptr;
+  HydroTotals* d_hydro = nullptr;
+  double hydro_bud[SM_HYDRO_BUDGET_SLOTS] = {};   // budget of the last successful hydrology call (SM_FLAG_BUDGET)
+  bool hydro_bud_valid = false;
   LbmDev lbm = {};                // wind field (sm_lbm_create)
   int lbm_cur = 0;                // buffer holding the current populations
   RunCtl* h_ctl = nullptr;        // pinned
@@ -2106,7 +2125,9 @@ int sm_wind_run_device(sm_context* ctx, int32_t n, const float* d_xy, int32_t ma
 }
 
 // ---- pooling hydrology ----------------------------------------------------------------------------
-// SM_HYDRO=warp | thread selects the executor of the flood phase and the seep pass
+// SM_HYDRO=warp | thread selects the executor of the flood phase and the seep pass.  A context created with
+// SM_FLAG_BUDGET runs the warp executor whatever SM_HYDRO says: the hydrology's budget lives only there, as the
+// batches' budget lives only in the warp sweep kernel.
 static bool hydro_warp() {
   const char* e = getenv("SM_HYDRO");
   if (e && strcmp(e, "warp") == 0) return true;
@@ -2119,7 +2140,7 @@ static int hydro_ready(sm_context* ctx) {
   if (ctx->nranks > 1) return fail(ctx, SM_ERR_INVALID, "pooling hydrology is not available on a sharded context");
   CK(cudaSetDevice(ctx->cfg.device));
   if (!ctx->d_hydro) {
-    CK(cudaMalloc(&ctx->d_hydro, sizeof(HydroCount)));
+    CK(cudaMalloc(&ctx->d_hydro, sizeof(HydroTotals)));
     CK(cudaFuncSetAttribute(k_hydro_flood, cudaFuncAttributeMaxDynamicSharedMemorySize, SM_HC_BYTES));
     CK(cudaFuncSetAttribute(k_hydro_seep, cudaFuncAttributeMaxDynamicSharedMemorySize, SM_HC_BYTES));
   }
@@ -2129,9 +2150,11 @@ static int hydro_ready(sm_context* ctx) {
   return SM_OK;
 }
 static int hydro_finish(sm_context* ctx, sm_hydro_stats* st) {
-  HydroCount hc;
+  HydroTotals tot;
+  const HydroCount& hc = tot.hc;
+  const bool budget = ctx->d.bud != nullptr;
   CK(cudaEventRecord(ctx->ev1, ctx->stream));
-  CK(cudaMemcpyAsync(&hc, ctx->d_hydro, sizeof(hc), cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaMemcpyAsync(&tot, ctx->d_hydro, budget ? sizeof(tot) : sizeof(hc), cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
   float ms = 0.f;
   CK(cudaEventElapsedTime(&ms, ctx->ev0, ctx->ev1));
@@ -2145,6 +2168,10 @@ static int hydro_finish(sm_context* ctx, sm_hydro_stats* st) {
   unsigned int err = 0;
   CK(cudaMemcpy(&err, &ctx->d.ctl->err, sizeof(err), cudaMemcpyDeviceToHost));
   if (err & (1u << 3)) return fail(ctx, SM_ERR_POOL, "section pool exhausted (sections were dropped)");
+  if (budget) {
+    for (int k = 0; k < SM_HYDRO_BUDGET_SLOTS; k++) ctx->hydro_bud[k] = tot.bud[k];
+    ctx->hydro_bud_valid = true;
+  }
   return SM_OK;
 }
 int sm_water_flood(sm_context* ctx, sm_hydro_stats* st) {
@@ -2152,8 +2179,9 @@ int sm_water_flood(sm_context* ctx, sm_hydro_stats* st) {
   if (rc != SM_OK) return rc;
   if (ctx->cur_kind != KIND_WATER) return fail(ctx, SM_ERR_INVALID, "sm_water_flood: the last batch was not a water batch");
   CK(cudaEventRecord(ctx->ev0, ctx->stream));
-  if (hydro_warp()) k_hydro_flood_w<<<1, 32, 0, ctx->stream>>>(ctx->d, ctx->cur_n, ctx->d_hydro);
-  else k_hydro_flood<<<1, 32, SM_HC_BYTES, ctx->stream>>>(ctx->d, ctx->cur_n, ctx->d_hydro);
+  if (ctx->d.bud) k_hydro_flood_w<true><<<1, 32, 0, ctx->stream>>>(ctx->d, ctx->cur_n, ctx->d_hydro);
+  else if (hydro_warp()) k_hydro_flood_w<false><<<1, 32, 0, ctx->stream>>>(ctx->d, ctx->cur_n, ctx->d_hydro);
+  else k_hydro_flood<<<1, 32, SM_HC_BYTES, ctx->stream>>>(ctx->d, ctx->cur_n, &ctx->d_hydro->hc);
   ctx->launches++;
   CK(cudaGetLastError());
   return hydro_finish(ctx, st);
@@ -2176,8 +2204,9 @@ int sm_seep(sm_context* ctx, sm_hydro_stats* st) {
   CK(cudaEventRecord(ctx->evt0, ctx->stream));
   k_hydro_classify<<<ctx->num_sms * 8, 256, 0, ctx->stream>>>(ctx->d, am);
   CK(cudaEventRecord(ctx->evt1, ctx->stream));
-  if (hydro_warp()) k_hydro_seep_w<<<1, 32, 0, ctx->stream>>>(ctx->d, am, ctx->d_hydro);
-  else k_hydro_seep<<<1, 32, SM_HC_BYTES, ctx->stream>>>(ctx->d, am, ctx->d_hydro);
+  if (ctx->d.bud) k_hydro_seep_w<true><<<1, 32, 0, ctx->stream>>>(ctx->d, am, ctx->d_hydro);
+  else if (hydro_warp()) k_hydro_seep_w<false><<<1, 32, 0, ctx->stream>>>(ctx->d, am, ctx->d_hydro);
+  else k_hydro_seep<<<1, 32, SM_HC_BYTES, ctx->stream>>>(ctx->d, am, &ctx->d_hydro->hc);
   ctx->launches += 2;
   CK(cudaGetLastError());
   int rc2 = hydro_finish(ctx, st);
@@ -2186,6 +2215,16 @@ int sm_seep(sm_context* ctx, sm_hydro_stats* st) {
     if (cudaEventElapsedTime(&cms, ctx->evt0, ctx->evt1) == cudaSuccess) st->classify_ms = cms;
   }
   return rc2;
+}
+int sm_last_hydro_budget(sm_context* ctx, sm_hydro_budget* out) {
+  if (!out) return fail(ctx, SM_ERR_INVALID, "null argument");
+  if (!ctx->d.bud) return fail(ctx, SM_ERR_INVALID, "context was created without SM_FLAG_BUDGET");
+  if (!ctx->hydro_bud_valid) return fail(ctx, SM_ERR_INVALID, "no hydrology call yet");
+  const double* b = ctx->hydro_bud;
+  out->flood_sediment = b[0]; out->flood_cascade_net = b[1]; out->flood_water = b[2]; out->seeped = b[3];
+  out->to_particles = b[4]; out->transfer_net = b[5]; out->nested_eroded = b[6]; out->nested_deposited = b[7];
+  out->nested_cascade_net = b[8]; out->nested_discarded = b[9]; out->nested_clamped = b[10];
+  return SM_OK;
 }
 
 // stepping interface: *_begin runs the prologue only (spawn + bins), *_sweeps(k) resumes the batch
