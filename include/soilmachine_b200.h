@@ -60,6 +60,8 @@ typedef struct sm_config {
 } sm_config;
 #define SM_FLAG_BUDGET 1      /* keep the per-particle mass budget (sm_last_budget) and the hydrology's
                                  (sm_last_hydro_budget); a few % slower */
+#define SM_FLAG_CELL_BUDGET 2 /* with SM_FLAG_BUDGET: also keep the per-cell maps of the last batch
+                                 (sm_last_cell_budget); 24 B per cell */
 
 /* Per-call counters (all accumulated over the call). */
 typedef struct sm_stats {
@@ -98,7 +100,7 @@ int sm_sync(sm_context* ctx);
  * change its strip again until the other ranks' calls have returned (a batch is safe: its ranks meet in a barrier
  * before any of them writes).  The pooling hydrology and the single-cell calls that change the map return
  * SM_ERR_INVALID on a sharded context. */
-#define SM_PEER_ARRAYS 20
+#define SM_PEER_ARRAYS 21
 #define SM_PEER_SLOTS 24
 typedef struct sm_peer_blob {
   uint64_t ptr[SM_PEER_SLOTS];
@@ -217,6 +219,30 @@ int sm_last_budget(sm_context* ctx, sm_budget* budget);
 /* the raw accumulators, 6 per particle (order as in sm_budget), for reductions over the ranks of a sharded map:
  * exactly one rank holds a particle's sums, the others hold zeros */
 int sm_budget_particles(sm_context* ctx, int32_t n, double* out6n);
+/* Per-cell maps of the mass budget of the last batch (contexts created with SM_FLAG_BUDGET | SM_FLAG_CELL_BUDGET):
+ * where the batch eroded, deposited and moved height by cascades.  Three f64 per cell of this context's strip, cell
+ * order x*dimy + y ((x - x0)*dimy + y on a sharded map, as sm_download_height); any pointer may be NULL.
+ *   eroded       at the particle's ipos, around the erosion remove (water.h:98-100; wind.h:109, signed)
+ *   deposited    water: at ipos (water.h:109); wind: at npos, then at ipos, each add measured at its own cell
+ *                (wind.h:123-124)
+ *   cascade_net  at both cells of every transfer of Particle::cascade (particle.h:87-92), nested re-cascades
+ *                included: the higher cell gets its own change of height and the lower cell its own
+ * Each delta is a column height (floor + top size) read right before and right after the column operation, at the
+ * measurement points of sm_budget, credited to the cell whose height was read.  A cell's total starts at +0.0 when
+ * the batch begins and every delta is added in execution order; two particle-steps that touch a cell are ordered by
+ * the lockstep schedule, so the maps are deterministic and bit-identical to a sequential restatement on any schedule
+ * and any number of ranks (the particle budget adds a transfer's two cells as one sum, the maps add each cell on its
+ * own).  Per cell: height after - height before = deposited - eroded + cascade_net, to rounding; cells no step
+ * touched hold exactly 0.0.
+ * Scope: the last batch.  sm_water_run / sm_wind_run / *_run_device / *_begin reset the maps, *_sweeps adds onto them;
+ * sm_water_flood, sm_seep and the single-cell calls never touch them, so the particles the pooling hydrology spawns
+ * are not in the maps.  On a sharded map a step also writes into the neighbouring ranks' maps: every rank's batch must
+ * have completed (sm_sync on every rank, then a host barrier) before the maps are read.
+ * Memory: 24 B per cell (403 MB at 4096^2, 1.6 GB at 8192^2).  Only the warp sweep kernel keeps the maps.
+ * SM_ERR_INVALID without SM_FLAG_CELL_BUDGET, before the first batch, or when the last batch ran on a kernel without
+ * the maps (SM_KERNEL=thread).  sm_create refuses SM_FLAG_CELL_BUDGET without SM_FLAG_BUDGET, sm_peer_attach ranks
+ * that disagree on it. */
+int sm_last_cell_budget(sm_context* ctx, double* eroded, double* deposited, double* cascade_net);
 
 /* Stepping interface for parity tests: begin a batch, advance k sweeps, read particle state. */
 int sm_water_begin(sm_context* ctx, int32_t n, const float* spawn_xy);

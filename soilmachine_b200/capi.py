@@ -36,7 +36,7 @@ SYMBOLS = [
     "sm_wind_sweeps", "sm_wind_state", "sm_launch_count", "sm_device_alloc", "sm_device_free",
     "sm_device_upload", "sm_timer_start", "sm_timer_stop", "sm_set_soil_colors", "sm_mesh_update",
     "sm_mesh_device_ptr", "sm_export_height", "sm_export_color", "sm_create_sharded", "sm_shard_range",
-    "sm_peer_export", "sm_peer_attach", "sm_parse_soil_file", "sm_water_flood", "sm_seep", "sm_last_budget", "sm_budget_particles", "sm_last_hydro_budget", "sm_lbm_create", "sm_lbm_set_boundary", "sm_lbm_init",
+    "sm_peer_export", "sm_peer_attach", "sm_parse_soil_file", "sm_water_flood", "sm_seep", "sm_last_budget", "sm_budget_particles", "sm_last_cell_budget", "sm_last_hydro_budget", "sm_lbm_create", "sm_lbm_set_boundary", "sm_lbm_init",
     "sm_lbm_step", "sm_lbm_get", "sm_lbm_advect", "sm_wind_use_lbm",
 ]
 
@@ -80,6 +80,9 @@ class HydroBudget(C.Structure):
 
     def asdict(self):
         return {k: getattr(self, k) for k, _ in self._fields_}
+
+
+CELL_TERMS = ("eroded", "deposited", "cascade_net")     # sm_last_cell_budget
 
 
 class SoilMachineError(RuntimeError):
@@ -146,11 +149,12 @@ class Context:
     """One sm_context (one GPU, or one rank of a sharded map)."""
 
     def __init__(self, dimx, dimy, scale=80, device=0, pool_capacity=0, max_particles=0,
-                 nranks=1, rank=0, share=1, budget=False):
+                 nranks=1, rank=0, share=1, budget=False, cell_budget=False):
+        """cell_budget=True keeps the per-cell budget maps as well (SM_FLAG_BUDGET | SM_FLAG_CELL_BUDGET)"""
         self.lib = load()
         self.dimx, self.dimy, self.scale = int(dimx), int(dimy), int(scale)
-        cfg = Config(self.dimx, self.dimy, self.scale, int(device), int(pool_capacity), int(max_particles),
-                     1 if budget else 0)                       # SM_FLAG_BUDGET
+        flags = 3 if cell_budget else (1 if budget else 0)     # SM_FLAG_BUDGET | SM_FLAG_CELL_BUDGET
+        cfg = Config(self.dimx, self.dimy, self.scale, int(device), int(pool_capacity), int(max_particles), flags)
         h = C.c_void_p()
         if nranks == 1:
             rc = self.lib.sm_create(C.byref(cfg), C.byref(h))
@@ -358,6 +362,13 @@ class Context:
         b = Budget()
         self._ck(self.lib.sm_last_budget(self.h, C.byref(b)))
         return b
+
+    def last_cell_budget(self):
+        """per-cell budget maps of the last batch (context created with cell_budget=True): a dict of three float64
+        arrays "eroded", "deposited", "cascade_net" of shape (x1 - x0, dimy)"""
+        out = {k: np.zeros(self.cells) for k in CELL_TERMS}
+        self._ck_strict(self.lib.sm_last_cell_budget(self.h, *[_p(out[k], C.c_double) for k in CELL_TERMS]))
+        return {k: v.reshape(self.x1 - self.x0, self.dimy) for k, v in out.items()}
 
     # ---- wind field (D3Q19 lattice Boltzmann) ----
     def lbm_create(self, nx, ny, nz):

@@ -49,6 +49,14 @@
 // Budget identity: d(sum of heights) = deposited - eroded + cascade_net (+ rounding), checked by the tests.
 #define SM_BUDGET_SLOTS 6
 
+// Per-cell maps of the mass budget (SM_FLAG_CELL_BUDGET): terms 0 eroded, 1 deposited, 2 cascade_net, measured where
+// slots 0-2 above are, but each delta is credited to the cell whose height was read (a cascade transfer credits the
+// higher and the lower cell separately).  A backing that declares `static constexpr bool kCellBudget = true` gets
+// cell_budget(term, x, y, delta) at every measurement point, called by the lane that mutates the column, in execution
+// order; a backing without the member (the host emulation's HostBack, the hydrology's HydroBack) compiles as before.
+template <class B, class = void> struct CellBudgetOf { static constexpr bool value = false; };
+template <class B> struct CellBudgetOf<B, decltype(void(B::kCellBudget))> { static constexpr bool value = B::kCellBudget; };
+
 // per-warp scratch (shared memory on the device)
 struct
 #if defined(__CUDACC__)
@@ -100,7 +108,8 @@ SM_HD void wind_field_pspeed(const WindField& f, float px, float py, double heig
 // B provides: dimx() dimy() scale(), soilp(t) -> const SoilDev*, cell_ptr(x, y) -> Sec32* (global record),
 // focus(x, y), pool_load/pool_store/pool_alloc/pool_free, wfreq(ind) wtrack(ind) windfreq(ind),
 // set_wtrack(ind, v) set_windfreq(ind, v), note_transfer(), pspeed(px, py, height, out3), kBudget, kHydroHooks
-// (+ air_mark(rec, x, y), wet_mark(x, y), volume_factor() when kHydroHooks).
+// (+ air_mark(rec, x, y), wet_mark(x, y), volume_factor() when kHydroHooks; + cell_budget(term, x, y, d) when it
+// declares kCellBudget = true).
 // ax..f_track are warp-uniform: every lane holds the same values and updates them identically.
 template <class B> struct CoopWin {
   B& b;
@@ -110,6 +119,7 @@ template <class B> struct CoopWin {
   bool has_b;
   float f_freq, f_track;
   static constexpr bool kBudget = B::kBudget;
+  static constexpr bool kCellBudget = CellBudgetOf<B>::value;
   SM_HD CoopWin(B& b_, CoopScratch* s_) : b(b_), s(s_), ax(0), ay(0), bx(0), by(0), valid(0), dirtym(0), has_b(false),
                                           f_freq(0.f), f_track(0.f) {}
   SM_HD int dimx() const { return b.dimx(); }
@@ -199,6 +209,10 @@ template <class B> struct CoopWin {
   SM_HD void dirty_rec(Sec32* r, int x, int y) { dirty_rec(r); if (B::kHydroHooks) b.air_mark(r, x, y); }
   SM_HD void wet_mark(int x, int y) { if (B::kHydroHooks) b.wet_mark(x, y); }
   SM_HD double volume_factor() const { return b.volume_factor(); }
+  // per-cell budget maps: add `d` to term `term` of cell (x, y) (single lane; nothing without kCellBudget)
+  SM_HD void cell_budget(int term, int x, int y, double d) {
+    if constexpr (kCellBudget) b.cell_budget(term, x, y, d);
+  }
   // write the modified records back: one record per lane
   template <class W> SM_HD void flush(W& w) {
     const uint32_t m = dirtym;
@@ -301,7 +315,12 @@ template <int DEPTH, class W, class A> struct CascadeCoop {
         const bool re = col_remove(a, *tr, (double)transfer) != 0;          // :90-91
         a.focus(ctop ? nx : cx, ctop ? ny : cy);
         col_add(a, *br, (double)transfer, casc);                            // :92
-        if (A::kBudget) a.s->acc[2] += (rec_height(*tr) - ht0) + (rec_height(*br) - hb0);
+        if (A::kBudget) {
+          const double dt = rec_height(*tr) - ht0, db = rec_height(*br) - hb0;
+          a.s->acc[2] += dt + db;
+          a.cell_budget(2, ctop ? cx : nx, ctop ? cy : ny, dt);
+          a.cell_budget(2, ctop ? nx : cx, ctop ? ny : cy, db);
+        }
         a.s->u = re ? 1u : 0u;
       });
       a.touched(w, pc, cx, cy);
@@ -404,7 +423,7 @@ template <class W, class A> SM_HD int water_interact_coop(W& w, A& a, WaterP& p,
       double diff = col_remove(a, *ir, amount);
       SM_UNROLL1
       while (fabs(diff) > 1E-8) diff = col_remove(a, *ir, diff);
-      if (A::kBudget) a.s->acc[0] += h0 - rec_height(*ir);
+      if (A::kBudget) { const double d = h0 - rec_height(*ir); a.s->acc[0] += d; a.cell_budget(0, ix, iy, d); }
     });
     a.dirty_rec(ir);
   } else if (cdiff < 0) {                                           // :105-110
@@ -416,7 +435,7 @@ template <class W, class A> SM_HD int water_interact_coop(W& w, A& a, WaterP& p,
       const double h0 = A::kBudget ? rec_height(*ir) : 0.0;
       a.focus(ix, iy);
       col_add(a, *ir, amount, what);
-      if (A::kBudget) a.s->acc[1] += rec_height(*ir) - h0;
+      if (A::kBudget) { const double d = rec_height(*ir) - h0; a.s->acc[1] += d; a.cell_budget(1, ix, iy, d); }
     });
     a.dirty_rec(ir);
   }
@@ -517,7 +536,12 @@ template <class W, class A> SM_HD int wind_interact_coop(W& w, A& a, WindP& p, c
         const double h0 = A::kBudget ? rec_height(*ir) : 0.0;
         a.focus(ix, iy);
         a.s->d = col_remove(a, *ir, amount);                        // :109
-        if (A::kBudget) { a.s->acc[0] += h0 - rec_height(*ir); if (amount < 0.0) a.s->acc[5] += amount; }
+        if (A::kBudget) {
+          const double d = h0 - rec_height(*ir);
+          a.s->acc[0] += d;
+          a.cell_budget(0, ix, iy, d);
+          if (amount < 0.0) a.s->acc[5] += amount;
+        }
       });
       a.dirty_rec(ir);
       p.sediment += (amount - a.s->d);                              // :110
@@ -533,10 +557,15 @@ template <class W, class A> SM_HD int wind_interact_coop(W& w, A& a, WindP& p, c
       double h0 = A::kBudget ? rec_height(*nr) : 0.0;
       a.focus(nx, ny);
       col_add(a, *nr, amount, what);                                // :123
-      if (A::kBudget) { a.s->acc[1] += rec_height(*nr) - h0; h0 = rec_height(*ir); }
+      if (A::kBudget) {
+        const double d = rec_height(*nr) - h0;
+        a.s->acc[1] += d;
+        a.cell_budget(1, nx, ny, d);
+        h0 = rec_height(*ir);
+      }
       a.focus(ix, iy);
       col_add(a, *ir, amount, what);                                // :124
-      if (A::kBudget) a.s->acc[1] += rec_height(*ir) - h0;
+      if (A::kBudget) { const double d = rec_height(*ir) - h0; a.s->acc[1] += d; a.cell_budget(1, ix, iy, d); }
     });
     a.dirty_rec(nr);
     a.dirty_rec(ir);

@@ -1329,6 +1329,10 @@ struct sm_context {
   HydroTotals* d_hydro = nullptr;
   double hydro_bud[SM_HYDRO_BUDGET_SLOTS] = {};   // budget of the last successful hydrology call (SM_FLAG_BUDGET)
   bool hydro_bud_valid = false;
+  // per-cell budget maps (SM_FLAG_CELL_BUDGET): 3 f64 per cell of the strip, interleaved; every rank's, by rank
+  double* d_cells = nullptr;
+  CellMaps cells_of = {};
+  int cells_state = 0;            // 0 no batch yet, 1 the maps cover the last batch, 2 it ran on a kernel without them
   LbmDev lbm = {};                // wind field (sm_lbm_create)
   int lbm_cur = 0;                // buffer holding the current populations
   RunCtl* h_ctl = nullptr;        // pinned
@@ -1378,7 +1382,7 @@ void sm_destroy(sm_context* ctx) {
   for (int i = 0; i < 3; i++) cudaFree(d.lmask[i]);
   for (int i = 0; i < 2; i++) { cudaFree(d.head[i]); cudaFree(d.node[i]); }
   cudaFree(ctx->d_verts); cudaFree(ctx->d_colors); cudaFree(d.dbg);
-  cudaFree(ctx->d_act); cudaFree(ctx->d_hydro);
+  cudaFree(ctx->d_act); cudaFree(ctx->d_hydro); cudaFree(ctx->d_cells);
   cudaFree(ctx->lbm.F[0]); cudaFree(ctx->lbm.F[1]); cudaFree(ctx->lbm.B); cudaFree(ctx->lbm.RHO); cudaFree(ctx->lbm.V);
   cudaFree(ctx->d_spawn); cudaFree(ctx->d_scratch); cudaFree(ctx->d_iscratch); cudaFree(ctx->d_cellres);
   if (ctx->h_ctl) cudaFreeHost(ctx->h_ctl);
@@ -1408,6 +1412,10 @@ static int create_impl(const sm_config* cfg, int nranks, int rank, int share, sm
   if (!cfg || !out || cfg->dimx < 2 || cfg->dimy < 2 || cfg->dimx > 16384 || cfg->dimy > 16384 ||
       nranks < 1 || nranks > SM_MAX_RANKS || rank < 0 || rank >= nranks || share < 1) {
     g_create_err = "sm_create: invalid configuration";
+    return SM_ERR_INVALID;
+  }
+  if ((cfg->flags & SM_FLAG_CELL_BUDGET) && !(cfg->flags & SM_FLAG_BUDGET)) {
+    g_create_err = "sm_create: SM_FLAG_CELL_BUDGET needs SM_FLAG_BUDGET";
     return SM_ERR_INVALID;
   }
   // x-strips of equal width (a multiple of the largest bin edge, 16 cells)
@@ -1464,6 +1472,11 @@ static int create_impl(const sm_config* cfg, int nranks, int rank, int share, sm
     if (cfg->flags & SM_FLAG_BUDGET) {
       CK(cudaMalloc(&d.bud, N * SM_BUDGET_SLOTS * sizeof(double)));
       CK(cudaMemsetAsync(d.bud, 0, N * SM_BUDGET_SLOTS * sizeof(double), ctx->stream));
+    }
+    if (cfg->flags & SM_FLAG_CELL_BUDGET) {
+      CK(cudaMalloc(&ctx->d_cells, LC * 3 * sizeof(double)));
+      CK(cudaMemsetAsync(ctx->d_cells, 0, LC * 3 * sizeof(double), ctx->stream));
+      if (nranks == 1) ctx->cells_of.p[0] = ctx->d_cells;    // sharded: every rank's, at sm_peer_attach
     }
     CK(cudaMemsetAsync(d.fin, 0, N * 4, ctx->stream)); CK(cudaMemsetAsync(d.mv, 0, N * 8, ctx->stream));
     d.nbx = (cfg->dimx + SM_MIN_BIN - 1) / SM_MIN_BIN; d.nby = (cfg->dimy + SM_MIN_BIN - 1) / SM_MIN_BIN;
@@ -1527,6 +1540,7 @@ static void own_ptrs(sm_context* ctx, void** p) {
   p[0] = d.top; p[1] = d.pool; p[2] = d.ringbuf[0]; p[3] = d.ringbuf[1]; p[4] = d.ctl; p[5] = d.pa; p[6] = d.pb;
   p[7] = d.pc; p[8] = d.alive; p[9] = d.done; p[10] = d.head[0]; p[11] = d.head[1]; p[12] = d.node[0]; p[13] = d.node[1];
   p[14] = d.ringbuf[2]; p[15] = d.bud; p[16] = d.fin; p[17] = d.lmask[0]; p[18] = d.lmask[1]; p[19] = d.lmask[2];
+  p[20] = ctx->d_cells;
 }
 static void fill_peer(PeerPtrs& P, void* const* p, unsigned long long pool_cap) {
   P.top = (Sec32*)p[0]; P.pool = (Sec32*)p[1]; P.ringbuf[0] = (uint32_t*)p[2]; P.ringbuf[1] = (uint32_t*)p[3];
@@ -1545,7 +1559,7 @@ int sm_peer_export(sm_context* ctx, sm_peer_blob* out) {
   own_ptrs(ctx, p);
   for (int i = 0; i < SM_PEER_ARRAYS; i++) {
     out->ptr[i] = (uint64_t)(uintptr_t)p[i];
-    if (!p[i]) continue;                      // optional array (mass budget) not allocated
+    if (!p[i]) continue;                      // optional array (mass budget, per-cell maps) not allocated
     cudaIpcMemHandle_t h;
     CK(cudaIpcGetMemHandle(&h, p[i]));
     static_assert(sizeof(h) == 64, "cudaIpcMemHandle_t is 64 bytes");
@@ -1558,6 +1572,9 @@ int sm_peer_export(sm_context* ctx, sm_peer_blob* out) {
 }
 int sm_peer_attach(sm_context* ctx, const sm_peer_blob* blobs, int32_t nblobs, int32_t use_ipc) {
   if (!blobs || nblobs != ctx->nranks) return fail(ctx, SM_ERR_INVALID, "sm_peer_attach: one blob per rank");
+  for (int q = 0; q < nblobs; q++)   // slot 20: the per-cell budget maps; a step writes into its neighbours' maps
+    if ((blobs[q].ptr[20] != 0) != (ctx->d_cells != nullptr))
+      return fail(ctx, SM_ERR_INVALID, "sm_peer_attach: the ranks disagree on SM_FLAG_CELL_BUDGET");
   CK(cudaSetDevice(ctx->cfg.device));
   for (int q = 0; q < ctx->nranks; q++) {
     const sm_peer_blob& b = blobs[q];
@@ -1585,6 +1602,7 @@ int sm_peer_attach(sm_context* ctx, const sm_peer_blob* blobs, int32_t nblobs, i
       }
     }
     fill_peer(ctx->d.peer[q], p, b.pool_cap);
+    ctx->cells_of.p[q] = (double*)p[20];
   }
   ctx->peers_attached = true;
   return SM_OK;
@@ -1970,6 +1988,9 @@ static int launch_run(sm_context* ctx, int kind, int n, const float* d_spawn, in
     if (e && strcmp(e, "thread") == 0) use_coop = false;
     if (e && strcmp(e, "warp") == 0) use_coop = true;
   }
+  // per-cell maps: only the warp kernel keeps them; a batch any of whose launches ran without them has no maps
+  if (ctx->d_cells && !use_coop) ctx->cells_state = 2;
+  else if (ctx->d_cells && ctx->cells_state == 0) ctx->cells_state = 1;
   if (use_coop) {
     const int sw_warps = kind == KIND_WIND ? SwShape<KIND_WIND>::WARPS : SwShape<KIND_WATER>::WARPS;
     const int cthreads = sw_warps * 32;
@@ -1981,15 +2002,21 @@ static int launch_run(sm_context* ctx, int kind, int n, const float* d_spawn, in
       const char* e = getenv("SM_EXACT");
       exact = (((e ? atoi(e) : SM_DEFAULT_EXACT) >> kind) & 1) != 0;
     }
-    void* const fns[16] = {(void*)k_sweep<KIND_WATER, false, false, false>, (void*)k_sweep<KIND_WIND, false, false, false>,
-                           (void*)k_sweep<KIND_WATER, true, false, false>,  (void*)k_sweep<KIND_WIND, true, false, false>,
-                           (void*)k_sweep<KIND_WATER, false, true, false>,  (void*)k_sweep<KIND_WIND, false, true, false>,
-                           (void*)k_sweep<KIND_WATER, true, true, false>,   (void*)k_sweep<KIND_WIND, true, true, false>,
-                           (void*)k_sweep<KIND_WATER, false, false, true>,  (void*)k_sweep<KIND_WIND, false, false, true>,
-                           (void*)k_sweep<KIND_WATER, true, false, true>,   (void*)k_sweep<KIND_WIND, true, false, true>,
-                           (void*)k_sweep<KIND_WATER, false, true, true>,   (void*)k_sweep<KIND_WIND, false, true, true>,
-                           (void*)k_sweep<KIND_WATER, true, true, true>,    (void*)k_sweep<KIND_WIND, true, true, true>};
-    void* fn = fns[(exact ? 8 : 0) + (budget ? 4 : 0) + (multi ? 2 : 0) + (kind == KIND_WATER ? 0 : 1)];
+    void* const fns[16] = {(void*)k_sweep<KIND_WATER, false, false, false, false>, (void*)k_sweep<KIND_WIND, false, false, false, false>,
+                           (void*)k_sweep<KIND_WATER, true, false, false, false>,  (void*)k_sweep<KIND_WIND, true, false, false, false>,
+                           (void*)k_sweep<KIND_WATER, false, true, false, false>,  (void*)k_sweep<KIND_WIND, false, true, false, false>,
+                           (void*)k_sweep<KIND_WATER, true, true, false, false>,   (void*)k_sweep<KIND_WIND, true, true, false, false>,
+                           (void*)k_sweep<KIND_WATER, false, false, true, false>,  (void*)k_sweep<KIND_WIND, false, false, true, false>,
+                           (void*)k_sweep<KIND_WATER, true, false, true, false>,   (void*)k_sweep<KIND_WIND, true, false, true, false>,
+                           (void*)k_sweep<KIND_WATER, false, true, true, false>,   (void*)k_sweep<KIND_WIND, false, true, true, false>,
+                           (void*)k_sweep<KIND_WATER, true, true, true, false>,    (void*)k_sweep<KIND_WIND, true, true, true, false>};
+    // with the per-cell maps (SM_FLAG_CELL_BUDGET, which implies the budget)
+    void* const fns_cells[8] = {(void*)k_sweep<KIND_WATER, false, true, false, true>, (void*)k_sweep<KIND_WIND, false, true, false, true>,
+                                (void*)k_sweep<KIND_WATER, true, true, false, true>,  (void*)k_sweep<KIND_WIND, true, true, false, true>,
+                                (void*)k_sweep<KIND_WATER, false, true, true, true>,  (void*)k_sweep<KIND_WIND, false, true, true, true>,
+                                (void*)k_sweep<KIND_WATER, true, true, true, true>,   (void*)k_sweep<KIND_WIND, true, true, true, true>};
+    void* fn = ctx->d_cells ? fns_cells[(exact ? 4 : 0) + (multi ? 2 : 0) + (kind == KIND_WATER ? 0 : 1)]
+                            : fns[(exact ? 8 : 0) + (budget ? 4 : 0) + (multi ? 2 : 0) + (kind == KIND_WATER ? 0 : 1)];
     // dynamic shared memory: the live mask of the batch and its popcount prefix (2 x n/32 words per block)
     const size_t csmem = (size_t)2 * (((size_t)std::max(n, 1) + 31) / 32) * sizeof(unsigned int);
     if (csmem > 40 * 1024) CK(cudaFuncSetAttribute((const void*)fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)csmem));
@@ -2003,7 +2030,8 @@ static int launch_run(sm_context* ctx, int kind, int n, const float* d_spawn, in
     int ms = max_sweeps;
     if (ms <= 0) ms = -1;
     if (max_sweeps == SM_SWEEPS_NONE) ms = 0;
-    void* cargs[] = {&dd, &n, (void*)&d_spawn, &ms};
+    CellMaps cm = ctx->cells_of;
+    void* cargs[] = {&dd, &n, (void*)&d_spawn, &ms, &cm};
     CK(cudaMemsetAsync(ctx->d.ctl, 0, 4 * sizeof(unsigned int), ctx->stream));  // barrier + alive_slot[3]
     CK(cudaMemsetAsync(&ctx->d.ctl->ticket[0], 0, 3 * sizeof(unsigned int), ctx->stream));
     for (int i = 0; i < 3; i++)      // the kernel's prologue sets the bits of the live particles
@@ -2067,6 +2095,16 @@ int sm_last_stats(sm_context* ctx, sm_stats* st) {
   return SM_OK;
 }
 
+// a new batch (*_run, *_run_device, *_begin): the per-cell maps start from +0.0; *_sweeps adds onto them
+static int new_batch(sm_context* ctx, int kind, int n) {
+  ctx->cur_kind = kind; ctx->cur_n = n;
+  if (ctx->d_cells) {
+    ctx->cells_state = 0;
+    CK(cudaMemsetAsync(ctx->d_cells, 0, ctx->lcells * 3 * sizeof(double), ctx->stream));
+  }
+  return SM_OK;
+}
+
 static int run_host(sm_context* ctx, int kind, int n, const float* spawn_xy, int max_sweeps, sm_stats* st) {
   if (n > 0 && !spawn_xy) return fail(ctx, SM_ERR_INVALID, "null spawn list");
   if (ctx->nranks > 1 && ctx->share > 1)
@@ -2076,7 +2114,8 @@ static int run_host(sm_context* ctx, int kind, int n, const float* spawn_xy, int
   if (n) CK(cudaMemcpyAsync(ctx->d_spawn, spawn_xy, (size_t)n * 8, cudaMemcpyHostToDevice, ctx->stream));
   int rc = zero_counters(ctx);
   if (rc != SM_OK) return rc;
-  ctx->cur_kind = kind; ctx->cur_n = n;
+  rc = new_batch(ctx, kind, n);
+  if (rc != SM_OK) return rc;
   rc = launch_run(ctx, kind, n, ctx->d_spawn, max_sweeps);
   if (rc != SM_OK) return rc;
   return sm_last_stats(ctx, st);
@@ -2105,6 +2144,21 @@ int sm_last_budget(sm_context* ctx, sm_budget* out) {
   return SM_OK;
 }
 
+int sm_last_cell_budget(sm_context* ctx, double* eroded, double* deposited, double* cascade_net) {
+  if (!ctx->d_cells) return fail(ctx, SM_ERR_INVALID, "context was created without SM_FLAG_CELL_BUDGET");
+  if (ctx->cells_state == 0) return fail(ctx, SM_ERR_INVALID, "no batch yet");
+  if (ctx->cells_state == 2)
+    return fail(ctx, SM_ERR_INVALID, "the last batch ran on a kernel without the per-cell maps (SM_KERNEL=thread)");
+  CK(cudaSetDevice(ctx->cfg.device));
+  CK(cudaStreamSynchronize(ctx->stream));
+  std::vector<double> m(ctx->lcells * 3);
+  CK(cudaMemcpy(m.data(), ctx->d_cells, m.size() * sizeof(double), cudaMemcpyDeviceToHost));
+  double* const out[3] = {eroded, deposited, cascade_net};
+  for (int k = 0; k < 3; k++)
+    if (out[k]) for (size_t i = 0; i < ctx->lcells; i++) out[k][i] = m[i * 3 + k];
+  return SM_OK;
+}
+
 int sm_water_run(sm_context* ctx, int32_t n, const float* xy, int32_t max_sweeps, sm_stats* st) {
   return run_host(ctx, KIND_WATER, n, xy, max_sweeps, st);
 }
@@ -2114,13 +2168,15 @@ int sm_wind_run(sm_context* ctx, int32_t n, const float* xy, int32_t max_sweeps,
 int sm_water_run_device(sm_context* ctx, int32_t n, const float* d_xy, int32_t max_sweeps) {
   int rc = zero_counters(ctx);
   if (rc != SM_OK) return rc;
-  ctx->cur_kind = KIND_WATER; ctx->cur_n = n;
+  rc = new_batch(ctx, KIND_WATER, n);
+  if (rc != SM_OK) return rc;
   return launch_run(ctx, KIND_WATER, n, d_xy, max_sweeps);
 }
 int sm_wind_run_device(sm_context* ctx, int32_t n, const float* d_xy, int32_t max_sweeps) {
   int rc = zero_counters(ctx);
   if (rc != SM_OK) return rc;
-  ctx->cur_kind = KIND_WIND; ctx->cur_n = n;
+  rc = new_batch(ctx, KIND_WIND, n);
+  if (rc != SM_OK) return rc;
   return launch_run(ctx, KIND_WIND, n, d_xy, max_sweeps);
 }
 

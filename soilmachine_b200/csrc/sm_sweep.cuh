@@ -51,10 +51,28 @@ struct WarpDev {
   __device__ __forceinline__ bool lead() const { return lane == 0; }
 };
 
+// Per-cell budget maps of every rank (SM_FLAG_CELL_BUDGET): 3 f64 per cell of the rank's strip, interleaved
+// (eroded, deposited, cascade_net), cell order (x - x0)*dimy + y.  A trailing parameter of k_sweep rather than a
+// DevCtx / PeerPtrs member, so that the layout every other kernel is compiled against stays as it is.
+struct CellMaps {
+  double* p[SM_MAX_RANKS];
+};
+
+// where DevBack<..., CELLS = true> finds the maps; empty otherwise, so that the other backings (HydroBack included)
+// keep their size and layout
+template <bool CELLS> struct CellMapsRef {
+  __device__ __forceinline__ explicit CellMapsRef(const CellMaps*) {}
+};
+template <> struct CellMapsRef<true> {
+  const CellMaps* cm;
+  __device__ __forceinline__ explicit CellMapsRef(const CellMaps* m) : cm(m) {}
+};
+
 // backing store of CoopWin on the device
-template <bool MULTI, bool BUDGET = false> struct DevBack {
+template <bool MULTI, bool BUDGET = false, bool CELLS = false> struct DevBack : CellMapsRef<CELLS> {
   static constexpr bool kBudget = BUDGET;
   static constexpr bool kHydroHooks = false;
+  static constexpr bool kCellBudget = CELLS;
   __device__ __forceinline__ void air_mark(Sec32*, int, int) {}
   __device__ __forceinline__ void wet_mark(int, int) {}
   __device__ __forceinline__ double volume_factor() const { return c.volume_factor; }
@@ -62,8 +80,16 @@ template <bool MULTI, bool BUDGET = false> struct DevBack {
   const SoilDev* s_soils;   // shared-memory copy of the soil table
   unsigned int phase;       // sweep number mod 3: frees go to ring[phase], allocations pop ring[(phase+1)%3]
   int cur_q;                // owner rank of the column the next col_* call works on
-  __device__ __forceinline__ DevBack(const DevCtx& ctx, const SoilDev* ss, unsigned int tag)
-      : c(ctx), s_soils(ss), phase(tag % 3u), cur_q(0) {}
+  __device__ __forceinline__ DevBack(const DevCtx& ctx, const SoilDev* ss, unsigned int tag, const CellMaps* m = nullptr)
+      : CellMapsRef<CELLS>(m), c(ctx), s_soils(ss), phase(tag % 3u), cur_q(0) {}
+  // One fire-and-forget f64 reduction (RED.ADD.F64.RN, the same rounding as `total += d`) into the owner's map: the
+  // warp does not wait for it.  Two steps that touch a cell are ordered by the conflict schedule and the reduction is
+  // issued by the lane that publishes the step, before its release, so each cell's additions land in execution order.
+  __device__ __forceinline__ void cell_budget(int term, int x, int y, double d) {
+    const int q = owner_of_x<MULTI>(c, x);
+    double* const m = this->cm->p[q];
+    atomicAdd(m + ((size_t)(x - q * c.strip_w) * c.dimy + y) * 3 + term, d);
+  }
   __device__ __forceinline__ int dimx() const { return c.dimx; }
   __device__ __forceinline__ int dimy() const { return c.dimy; }
   __device__ __forceinline__ int scale() const { return c.scale; }
@@ -309,10 +335,10 @@ template <class W, class A> __device__ __forceinline__ int do_move_coop_full(W& 
 template <int KIND> struct MidCoopType { typedef WaterMidCoop T; };
 template <> struct MidCoopType<KIND_WIND> { typedef WindMidCoop T; };
 
-template <int KIND, bool MULTI, bool BUDGET>
+template <int KIND, bool MULTI, bool BUDGET, bool CELLS>
 __device__ __forceinline__ int sweep_exact(const DevCtx& c, WarpSmem& ws, WarpDev& w, const SoilDev* s_soils,
                                            unsigned int tag, int pid, int ix, int iy, int myR,
-                                           typename PType<KIND>::T& p, bool edge) {
+                                           typename PType<KIND>::T& p, bool edge, const CellMaps* cm) {
   const int lane = w.lane;
   const unsigned int cnt = ws.cnt;
   const uint32_t ownpred = ws.pred[4];
@@ -346,8 +372,8 @@ __device__ __forceinline__ int sweep_exact(const DevCtx& c, WarpSmem& ws, WarpDe
     if (lane == 0) ws.n1[base >> 5] = left;
   }
   __syncwarp();
-  DevBack<MULTI, BUDGET> back(c, s_soils, tag);
-  CoopWin<DevBack<MULTI, BUDGET> > a(back, &ws.cs);
+  DevBack<MULTI, BUDGET, CELLS> back(c, s_soils, tag, cm);
+  CoopWin<DevBack<MULTI, BUDGET, CELLS> > a(back, &ws.cs);
   typename MidCoopType<KIND>::T mid;
   int r = do_move_coop(w, a, p, mid);
   if (r == SM_ALIVE) {
@@ -453,9 +479,10 @@ __device__ __forceinline__ unsigned int live_total(const unsigned int* __restric
   return total;
 }
 
-template <int KIND, bool MULTI, bool BUDGET, bool EXACT>
+// CELLS (with BUDGET only): also the per-cell budget maps, in `cm`; the other instantiations never read it.
+template <int KIND, bool MULTI, bool BUDGET, bool EXACT, bool CELLS>
 __global__ void __launch_bounds__(SwShape<KIND>::WARPS * 32, SwShape<KIND>::MINBLOCKS) k_sweep(DevCtx c, int n, const float* __restrict__ spawn,
-                                                                            int max_sweeps) {
+                                                                            int max_sweeps, const __grid_constant__ CellMaps cm) {
   typedef typename PType<KIND>::T P;
   constexpr int NWARPS = SwShape<KIND>::WARPS;
   __shared__ SoilDev s_soils[SM_MAX_SOILS];
@@ -618,15 +645,15 @@ __global__ void __launch_bounds__(SwShape<KIND>::WARPS * 32, SwShape<KIND>::MINB
         // (also for a particle with nothing in range: its mv word is what lets the particles behind it skip waits -
         // sending those down the conservative path makes the particles behind it wait longer)
         exact_now = ws.cnt <= SM_SW_NEARX && !(MULTI && ws.remote);
-        if (exact_now) r = sweep_exact<KIND, MULTI, BUDGET>(c, ws, w, s_soils, tag, pid, ix, iy, myR, p, edge);
+        if (exact_now) r = sweep_exact<KIND, MULTI, BUDGET, CELLS>(c, ws, w, s_soils, tag, pid, ix, iy, myR, p, edge, &cm);
       }
       if (!exact_now) {
         coop_wait<MULTI>(c, tag, tgt);
 #ifdef SM_PROFILE
         pc2 = clock64();
 #endif
-        DevBack<MULTI, BUDGET> back(c, s_soils, tag);
-        CoopWin<DevBack<MULTI, BUDGET> > a(back, &ws.cs);
+        DevBack<MULTI, BUDGET, CELLS> back(c, s_soils, tag, &cm);
+        CoopWin<DevBack<MULTI, BUDGET, CELLS> > a(back, &ws.cs);
 #ifdef SM_PROFILE
         long long pcm, pci;
         {

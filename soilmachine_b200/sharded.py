@@ -54,10 +54,12 @@ def sum_stats(stats):
 
 
 class VirtualShards:
-    def __init__(self, nranks, dimx, dimy, scale=80, device=0, max_particles=0, pool_capacity=0, budget=False):
+    def __init__(self, nranks, dimx, dimy, scale=80, device=0, max_particles=0, pool_capacity=0, budget=False,
+                 cell_budget=False):
         self.nranks, self.dimx, self.dimy = nranks, dimx, dimy
         self.ctx = [capi.Context(dimx, dimy, scale, device=device, max_particles=max_particles,
-                                 pool_capacity=pool_capacity, nranks=nranks, rank=r, share=nranks, budget=budget)
+                                 pool_capacity=pool_capacity, nranks=nranks, rank=r, share=nranks, budget=budget,
+                                 cell_budget=cell_budget)
                     for r in range(nranks)]
         blobs = [c.peer_export() for c in self.ctx]
         for c in self.ctx:
@@ -110,6 +112,13 @@ class VirtualShards:
 
     def wind_run(self, xy, max_sweeps=0):
         return self._run("wind", xy, max_sweeps)
+
+    def last_cell_budget(self):
+        """per-cell budget maps of the last batch over the whole map, shape (dimx, dimy): the strips concatenated
+        along x (a step also writes into its neighbours' strips, so every rank is synchronised first)"""
+        self.sync()
+        parts = [c.last_cell_budget() for c in self.ctx]
+        return {k: np.concatenate([p[k] for p in parts], axis=0) for k in capi.CELL_TERMS}
 
     # ---- read-only views of the whole map (meshing, export, queries, wind-field boundary) ----
     # Each of these reads other ranks' strips, so every rank's earlier work must have completed first: sync() does
@@ -173,15 +182,17 @@ class VirtualShards:
 class DistShard:
     """This process's rank of a map sharded over torch.distributed ranks (one GPU each)."""
 
-    def __init__(self, dimx, dimy, scale, device, max_particles=0, pool_capacity=0, share=1):
+    def __init__(self, dimx, dimy, scale, device, max_particles=0, pool_capacity=0, share=1, cell_budget=False):
         """share > 1: that many ranks (processes) run their kernels on the SAME device - used by the one-GPU
-        test of the CUDA-IPC path; every rank's grid must then be resident at the same time."""
+        test of the CUDA-IPC path; every rank's grid must then be resident at the same time.  cell_budget: keep
+        the per-cell budget maps (every rank must agree)."""
         import torch.distributed as dist
         self.dist = dist
         self.nranks, self.rank = dist.get_world_size(), dist.get_rank()
         self.dimx, self.dimy = dimx, dimy
         self.ctx = capi.Context(dimx, dimy, scale, device=device, max_particles=max_particles,
-                                pool_capacity=pool_capacity, nranks=self.nranks, rank=self.rank, share=share)
+                                pool_capacity=pool_capacity, nranks=self.nranks, rank=self.rank, share=share,
+                                cell_budget=cell_budget)
         mine = bytes(self.ctx.peer_export())
         blobs = [None] * self.nranks
         dist.all_gather_object(blobs, mine)
@@ -192,6 +203,12 @@ class DistShard:
         """launch this rank's sweep kernel (all ranks must call it), wait, return local stats"""
         (self.ctx.water_run_device if kind == "water" else self.ctx.wind_run_device)(d_xy, n, max_sweeps)
         return self.ctx.last_stats()
+
+    def last_cell_budget(self):
+        """this rank's strip of the per-cell budget maps, shape (x1 - x0, dimy); all ranks must call it (the other
+        ranks' steps write into this strip, so every rank's batch has to be complete first)"""
+        self._settle()
+        return self.ctx.last_cell_budget()
 
     # ---- read-only views of the whole map ----
     # The calls that read other ranks' strips first wait for this rank's work and then meet every other rank in a
