@@ -62,6 +62,8 @@ typedef struct sm_config {
                                  (sm_last_hydro_budget); a few % slower */
 #define SM_FLAG_CELL_BUDGET 2 /* with SM_FLAG_BUDGET: also keep the per-cell maps of the last batch
                                  (sm_last_cell_budget); 24 B per cell */
+#define SM_FLAG_HYDRO_CELL_BUDGET 4 /* with SM_FLAG_BUDGET: also keep the per-cell maps of the last sm_water_flood /
+                                       sm_seep call (sm_last_hydro_cell_budget); 32 B per cell; unsharded only */
 
 /* Per-call counters (all accumulated over the call). */
 typedef struct sm_stats {
@@ -236,7 +238,7 @@ int sm_budget_particles(sm_context* ctx, int32_t n, double* out6n);
  * touched hold exactly 0.0.
  * Scope: the last batch.  sm_water_run / sm_wind_run / *_run_device / *_begin reset the maps, *_sweeps adds onto them;
  * sm_water_flood, sm_seep and the single-cell calls never touch them, so the particles the pooling hydrology spawns
- * are not in the maps.  On a sharded map a step also writes into the neighbouring ranks' maps: every rank's batch must
+ * are not in the maps (sm_last_hydro_cell_budget has the floods' and the seep pass's own).  On a sharded map a step also writes into the neighbouring ranks' maps: every rank's batch must
  * have completed (sm_sync on every rank, then a host barrier) before the maps are read.
  * Memory: 24 B per cell (403 MB at 4096^2, 1.6 GB at 8192^2).  Only the warp sweep kernel keeps the maps.
  * SM_ERR_INVALID without SM_FLAG_CELL_BUDGET, before the first batch, or when the last batch ran on a kernel without
@@ -295,6 +297,32 @@ typedef struct sm_hydro_budget {
   double nested_clamped;
 } sm_hydro_budget;
 int sm_last_hydro_budget(sm_context* ctx, sm_hydro_budget* budget);
+/* Per-cell maps of the hydrology's mass budget (contexts created with SM_FLAG_BUDGET | SM_FLAG_HYDRO_CELL_BUDGET):
+ * where the last successful sm_water_flood or sm_seep call - the scope of sm_last_hydro_budget - changed the map.  Four
+ * f64 per cell, cell order x*dimy + y (as sm_download_height); any pointer may be NULL.
+ *   eroded       a nested particle's erosion, at its ipos                            (refines nested_eroded)
+ *   deposited    the flood's sediment add at the truncated ipos (water.h:133); a nested particle's deposit
+ *                                                                                    (flood_sediment + nested_deposited)
+ *   cascade_net  both cells of every terrain-cascade transfer, each its own change of height: the flood's cascade
+ *                (water.h:134) and the nested particles' cascades           (flood_cascade_net + nested_cascade_net)
+ *   water_net    the flood's Air add (water.h:138, +); every seep(cell), in a flood and in the seep pass (-, the
+ *                height removed); a whole water section leaving as a nested particle, at tpos (water.h:248, -); a
+ *                partial transfer, tpos and bpos each their own change (water.h:268-271)
+ *                                                         (flood_water - seeped - to_particles + transfer_net)
+ * Each delta is measured where the sm_hydro_budget sums are and credited to the cell whose height was read; the
+ * terms are heights, not materials (eroded can include water).  nested_discarded and nested_clamped have no cell.
+ * Every cell starts each call at +0.0 and its deltas are added in execution order, so the maps are deterministic.
+ * Per cell: height after - height before = deposited - eroded + cascade_net + water_net, to rounding; cells nothing
+ * touched hold exactly 0.0; summed over the cells each map equals its group of sm_hydro_budget terms, to rounding.
+ * The batch maps (sm_last_cell_budget) are not touched; the single-cell calls (sm_cell_seep, sm_cell_water_cascade)
+ * are not covered.  Memory: 32 B per cell of device memory (537 MB at 4096^2, 2.1 GB at 8192^2), zeroed by every
+ * sm_water_flood / sm_seep call inside its device_ms; this call stages the interleaved map through a 32 MB host buffer.
+ * SM_ERR_INVALID without SM_FLAG_HYDRO_CELL_BUDGET, before the first sm_water_flood / sm_seep call (a water batch alone
+ * does not count), or when the last of these calls failed (its maps were reset and are partial).  sm_create refuses
+ * the flag without SM_FLAG_BUDGET, and sm_create_sharded refuses it with nranks > 1: the pooling hydrology does not
+ * run on a sharded context. */
+int sm_last_hydro_cell_budget(sm_context* ctx, double* eroded, double* deposited, double* cascade_net,
+                              double* water_net);
 
 /* ---- wind field: D3Q19 lattice Boltzmann, TRT collision (source/include/lbmwind/) ------------------------------
  * The reference runs this as OpenGL compute shaders and only draws it (WindParticle keeps a constant prevailing

@@ -36,7 +36,7 @@ SYMBOLS = [
     "sm_wind_sweeps", "sm_wind_state", "sm_launch_count", "sm_device_alloc", "sm_device_free",
     "sm_device_upload", "sm_timer_start", "sm_timer_stop", "sm_set_soil_colors", "sm_mesh_update",
     "sm_mesh_device_ptr", "sm_export_height", "sm_export_color", "sm_create_sharded", "sm_shard_range",
-    "sm_peer_export", "sm_peer_attach", "sm_parse_soil_file", "sm_water_flood", "sm_seep", "sm_last_budget", "sm_budget_particles", "sm_last_cell_budget", "sm_last_hydro_budget", "sm_lbm_create", "sm_lbm_set_boundary", "sm_lbm_init",
+    "sm_peer_export", "sm_peer_attach", "sm_parse_soil_file", "sm_water_flood", "sm_seep", "sm_last_budget", "sm_budget_particles", "sm_last_cell_budget", "sm_last_hydro_budget", "sm_last_hydro_cell_budget", "sm_lbm_create", "sm_lbm_set_boundary", "sm_lbm_init",
     "sm_lbm_step", "sm_lbm_get", "sm_lbm_advect", "sm_wind_use_lbm",
 ]
 
@@ -83,6 +83,7 @@ class HydroBudget(C.Structure):
 
 
 CELL_TERMS = ("eroded", "deposited", "cascade_net")     # sm_last_cell_budget
+HYDRO_CELL_TERMS = ("eroded", "deposited", "cascade_net", "water_net")     # sm_last_hydro_cell_budget
 
 
 class SoilMachineError(RuntimeError):
@@ -149,11 +150,14 @@ class Context:
     """One sm_context (one GPU, or one rank of a sharded map)."""
 
     def __init__(self, dimx, dimy, scale=80, device=0, pool_capacity=0, max_particles=0,
-                 nranks=1, rank=0, share=1, budget=False, cell_budget=False):
-        """cell_budget=True keeps the per-cell budget maps as well (SM_FLAG_BUDGET | SM_FLAG_CELL_BUDGET)"""
+                 nranks=1, rank=0, share=1, budget=False, cell_budget=False, hydro_cell_budget=False):
+        """cell_budget=True keeps the per-cell budget maps of the batches as well (SM_FLAG_BUDGET | SM_FLAG_CELL_BUDGET),
+        hydro_cell_budget=True those of the hydrology calls (SM_FLAG_BUDGET | SM_FLAG_HYDRO_CELL_BUDGET)"""
         self.lib = load()
         self.dimx, self.dimy, self.scale = int(dimx), int(dimy), int(scale)
         flags = 3 if cell_budget else (1 if budget else 0)     # SM_FLAG_BUDGET | SM_FLAG_CELL_BUDGET
+        if hydro_cell_budget:
+            flags |= 1 | 4                                     # SM_FLAG_BUDGET | SM_FLAG_HYDRO_CELL_BUDGET
         cfg = Config(self.dimx, self.dimy, self.scale, int(device), int(pool_capacity), int(max_particles), flags)
         h = C.c_void_p()
         if nranks == 1:
@@ -420,6 +424,14 @@ class Context:
         b = HydroBudget()
         self._ck(self.lib.sm_last_hydro_budget(self.h, C.byref(b)))
         return b.asdict()
+
+    def last_hydro_cell_budget(self):
+        """per-cell maps of the hydrology's budget for the last water_flood or seep call (context created with
+        hydro_cell_budget=True): a dict of four float64 arrays "eroded", "deposited", "cascade_net", "water_net" of
+        shape (dimx, dimy)"""
+        out = {k: np.zeros(self.cells) for k in HYDRO_CELL_TERMS}
+        self._ck_strict(self.lib.sm_last_hydro_cell_budget(self.h, *[_p(out[k], C.c_double) for k in HYDRO_CELL_TERMS]))
+        return {k: v.reshape(self.dimx, self.dimy) for k, v in out.items()}
 
     def water_begin(self, xy):
         xy = np.ascontiguousarray(xy, np.float32)

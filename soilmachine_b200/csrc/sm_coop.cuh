@@ -53,7 +53,8 @@
 // slots 0-2 above are, but each delta is credited to the cell whose height was read (a cascade transfer credits the
 // higher and the lower cell separately).  A backing that declares `static constexpr bool kCellBudget = true` gets
 // cell_budget(term, x, y, delta) at every measurement point, called by the lane that mutates the column, in execution
-// order; a backing without the member (the host emulation's HostBack, the hydrology's HydroBack) compiles as before.
+// order; a backing without the member (the host emulation's HostBack, the hydrology's HydroBack<BUDGET>) compiles as
+// before.  The hydrology's HydroBack<true, true> routes the same calls into its own 4-term map (sm_hydro_coop.cuh).
 template <class B, class = void> struct CellBudgetOf { static constexpr bool value = false; };
 template <class B> struct CellBudgetOf<B, decltype(void(B::kCellBudget))> { static constexpr bool value = B::kCellBudget; };
 

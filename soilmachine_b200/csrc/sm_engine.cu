@@ -1219,12 +1219,36 @@ __global__ void __launch_bounds__(32) k_hydro_seep(DevCtx c, ActiveMap am, Hydro
 // nested particles on the cooperative step.  Records are accessed in place through L2 (a frame's nine records are
 // fetched by nine lanes at once, which is what the one-thread executor needs its shared-memory cache for).
 // BUDGET: the hydrology's mass budget (HydroScratchBudget::bud, sm_hydro_coop.cuh), for contexts created with SM_FLAG_BUDGET.
-template <bool BUDGET> struct HydroBack : DevBack<false, BUDGET> {
+// CELLS (with BUDGET): its per-cell maps, SM_HYDRO_CELL_TERMS f64 per cell interleaved (eroded, deposited, cascade_net,
+// water_net), cell order x*dimy + y, for contexts created with SM_FLAG_HYDRO_CELL_BUDGET.  The map pointer lives in an
+// empty-when-off base, so that HydroBack<BUDGET> keeps its size and layout.
+template <bool CELLS> struct HydroCellsRef {
+  __device__ __forceinline__ explicit HydroCellsRef(double*) {}
+};
+template <> struct HydroCellsRef<true> {
+  double* hcells;
+  __device__ __forceinline__ explicit HydroCellsRef(double* m) : hcells(m) {}
+};
+template <bool BUDGET, bool CELLS = false> struct HydroBack : DevBack<false, BUDGET>, HydroCellsRef<CELLS> {
+  static_assert(!CELLS || BUDGET, "the per-cell maps are measured by the budget instantiations");
   static constexpr bool kHydroHooks = true;
+  static constexpr bool kCellBudget = CELLS;
   ActiveMap act;
   bool marking;
-  __device__ __forceinline__ HydroBack(const DevCtx& ctx, const SoilDev* ss, const ActiveMap& am, bool mk)
-      : DevBack<false, BUDGET>(ctx, ss, 0u), act(am), marking(mk) {}
+  __device__ __forceinline__ HydroBack(const DevCtx& ctx, const SoilDev* ss, const ActiveMap& am, bool mk,
+                                       double* cells = nullptr)
+      : DevBack<false, BUDGET>(ctx, ss, 0u), HydroCellsRef<CELLS>(cells), act(am), marking(mk) {}
+  // One fire-and-forget f64 reduction (the rounding of `total += d`), as DevBack::cell_budget: the warp does not wait
+  // for it.  One lane of one warp issues them in program order, so each cell's additions land in execution order.  The
+  // map is device memory; saying so lets the compiler emit the global-space reduction (ATOMG/RED, no result used)
+  // instead of a generic-address atomic with a shared-memory fallback branch behind it.
+  __device__ __forceinline__ void cell_budget(int term, int x, int y, double d) {
+    if constexpr (CELLS) {
+      double* const m = this->hcells + ((size_t)x * this->c.dimy + y) * SM_HYDRO_CELL_TERMS + term;
+      __builtin_assume(__isGlobal(m));
+      atomicAdd(m, d);
+    }
+  }
   // single writer: only the lane that mutates columns calls these
   __device__ __forceinline__ void air_mark(Sec32* r, int x, int y) {
     if (marking && r->type == SM_AIR) active_mark_block(act, x, y, this->c.dimx, this->c.dimy);
@@ -1247,7 +1271,9 @@ template <bool BUDGET, class S> __device__ __forceinline__ void hydro_totals_out
   if constexpr (BUDGET)
     for (int k = 0; k < SM_HYDRO_BUDGET_SLOTS; k++) out->bud[k] = hx.bud[k];
 }
-template <bool BUDGET> __global__ void __launch_bounds__(32) k_hydro_flood_w(DevCtx c, int n, HydroTotals* out) {
+// `hcells`: the per-cell maps with CELLS (HydroBack), a trailing parameter so that DevCtx keeps its layout
+template <bool BUDGET, bool CELLS = false>
+__global__ void __launch_bounds__(32) k_hydro_flood_w(DevCtx c, int n, HydroTotals* out, double* hcells) {
   __shared__ SoilDev s_soils[SM_MAX_SOILS];
   __shared__ CoopScratch sc;
   __shared__ typename HydroScratchOf<BUDGET>::type hx;
@@ -1257,8 +1283,8 @@ template <bool BUDGET> __global__ void __launch_bounds__(32) k_hydro_flood_w(Dev
   __syncwarp();
   WarpDev w{lane};
   ActiveMap none{};
-  HydroBack<BUDGET> back(c, s_soils, none, false);
-  CoopWin<HydroBack<BUDGET> > a(back, &sc);
+  HydroBack<BUDGET, CELLS> back(c, s_soils, none, false, hcells);
+  CoopWin<HydroBack<BUDGET, CELLS> > a(back, &sc);
   HydroCount hc{};
   for (int base = 0; base < n; base += 32) {
     const int i = base + lane;
@@ -1280,7 +1306,8 @@ template <bool BUDGET> __global__ void __launch_bounds__(32) k_hydro_flood_w(Dev
   }
   if (lane == 0) hydro_totals_out<BUDGET>(out, hc, hx);
 }
-template <bool BUDGET> __global__ void __launch_bounds__(32) k_hydro_seep_w(DevCtx c, ActiveMap am, HydroTotals* out) {
+template <bool BUDGET, bool CELLS = false>
+__global__ void __launch_bounds__(32) k_hydro_seep_w(DevCtx c, ActiveMap am, HydroTotals* out, double* hcells) {
   __shared__ SoilDev s_soils[SM_MAX_SOILS];
   __shared__ CoopScratch sc;
   __shared__ typename HydroScratchOf<BUDGET>::type hx;
@@ -1289,8 +1316,8 @@ template <bool BUDGET> __global__ void __launch_bounds__(32) k_hydro_seep_w(DevC
   hydro_budget_zero<BUDGET>(hx, lane);
   __syncwarp();
   WarpDev w{lane};
-  HydroBack<BUDGET> back(c, s_soils, am, true);
-  CoopWin<HydroBack<BUDGET> > a(back, &sc);
+  HydroBack<BUDGET, CELLS> back(c, s_soils, am, true, hcells);
+  CoopWin<HydroBack<BUDGET, CELLS> > a(back, &sc);
   HydroCount hc{};
   const unsigned long long cells = am.ncells;
   for (unsigned long long cell = active_next(am, 0); cell < cells; cell = active_next(am, cell + 1)) {
@@ -1333,6 +1360,9 @@ struct sm_context {
   double* d_cells = nullptr;
   CellMaps cells_of = {};
   int cells_state = 0;            // 0 no batch yet, 1 the maps cover the last batch, 2 it ran on a kernel without them
+  // per-cell maps of the hydrology's budget (SM_FLAG_HYDRO_CELL_BUDGET): SM_HYDRO_CELL_TERMS f64 per cell, interleaved
+  double* d_hcells = nullptr;
+  int hcells_state = 0;           // 0 no hydrology call yet, 1 the maps cover the last call, 2 that call failed
   LbmDev lbm = {};                // wind field (sm_lbm_create)
   int lbm_cur = 0;                // buffer holding the current populations
   RunCtl* h_ctl = nullptr;        // pinned
@@ -1382,7 +1412,7 @@ void sm_destroy(sm_context* ctx) {
   for (int i = 0; i < 3; i++) cudaFree(d.lmask[i]);
   for (int i = 0; i < 2; i++) { cudaFree(d.head[i]); cudaFree(d.node[i]); }
   cudaFree(ctx->d_verts); cudaFree(ctx->d_colors); cudaFree(d.dbg);
-  cudaFree(ctx->d_act); cudaFree(ctx->d_hydro); cudaFree(ctx->d_cells);
+  cudaFree(ctx->d_act); cudaFree(ctx->d_hydro); cudaFree(ctx->d_cells); cudaFree(ctx->d_hcells);
   cudaFree(ctx->lbm.F[0]); cudaFree(ctx->lbm.F[1]); cudaFree(ctx->lbm.B); cudaFree(ctx->lbm.RHO); cudaFree(ctx->lbm.V);
   cudaFree(ctx->d_spawn); cudaFree(ctx->d_scratch); cudaFree(ctx->d_iscratch); cudaFree(ctx->d_cellres);
   if (ctx->h_ctl) cudaFreeHost(ctx->h_ctl);
@@ -1416,6 +1446,15 @@ static int create_impl(const sm_config* cfg, int nranks, int rank, int share, sm
   }
   if ((cfg->flags & SM_FLAG_CELL_BUDGET) && !(cfg->flags & SM_FLAG_BUDGET)) {
     g_create_err = "sm_create: SM_FLAG_CELL_BUDGET needs SM_FLAG_BUDGET";
+    return SM_ERR_INVALID;
+  }
+  if ((cfg->flags & SM_FLAG_HYDRO_CELL_BUDGET) && !(cfg->flags & SM_FLAG_BUDGET)) {
+    g_create_err = "sm_create: SM_FLAG_HYDRO_CELL_BUDGET needs SM_FLAG_BUDGET";
+    return SM_ERR_INVALID;
+  }
+  if ((cfg->flags & SM_FLAG_HYDRO_CELL_BUDGET) && nranks > 1) {
+    g_create_err = "sm_create_sharded: SM_FLAG_HYDRO_CELL_BUDGET needs the pooling hydrology, which does not run on a "
+                   "sharded context";
     return SM_ERR_INVALID;
   }
   // x-strips of equal width (a multiple of the largest bin edge, 16 cells)
@@ -1478,6 +1517,8 @@ static int create_impl(const sm_config* cfg, int nranks, int rank, int share, sm
       CK(cudaMemsetAsync(ctx->d_cells, 0, LC * 3 * sizeof(double), ctx->stream));
       if (nranks == 1) ctx->cells_of.p[0] = ctx->d_cells;    // sharded: every rank's, at sm_peer_attach
     }
+    if (cfg->flags & SM_FLAG_HYDRO_CELL_BUDGET)                // zeroed by every sm_water_flood / sm_seep
+      CK(cudaMalloc(&ctx->d_hcells, C * SM_HYDRO_CELL_TERMS * sizeof(double)));
     CK(cudaMemsetAsync(d.fin, 0, N * 4, ctx->stream)); CK(cudaMemsetAsync(d.mv, 0, N * 8, ctx->stream));
     d.nbx = (cfg->dimx + SM_MIN_BIN - 1) / SM_MIN_BIN; d.nby = (cfg->dimy + SM_MIN_BIN - 1) / SM_MIN_BIN;
     for (int i = 0; i < 2; i++) {
@@ -2183,7 +2224,7 @@ int sm_wind_run_device(sm_context* ctx, int32_t n, const float* d_xy, int32_t ma
 // ---- pooling hydrology ----------------------------------------------------------------------------
 // SM_HYDRO=warp | thread selects the executor of the flood phase and the seep pass.  A context created with
 // SM_FLAG_BUDGET runs the warp executor whatever SM_HYDRO says: the hydrology's budget lives only there, as the
-// batches' budget lives only in the warp sweep kernel.
+// batches' budget lives only in the warp sweep kernel.  SM_FLAG_HYDRO_CELL_BUDGET runs its CELLS instantiations.
 static bool hydro_warp() {
   const char* e = getenv("SM_HYDRO");
   if (e && strcmp(e, "warp") == 0) return true;
@@ -2228,6 +2269,14 @@ static int hydro_finish(sm_context* ctx, sm_hydro_stats* st) {
     for (int k = 0; k < SM_HYDRO_BUDGET_SLOTS; k++) ctx->hydro_bud[k] = tot.bud[k];
     ctx->hydro_bud_valid = true;
   }
+  if (ctx->d_hcells) ctx->hcells_state = 1;
+  return SM_OK;
+}
+// the per-cell maps start every call at +0.0; until the call has succeeded they are partial
+static int hydro_cells_reset(sm_context* ctx) {
+  if (!ctx->d_hcells) return SM_OK;
+  ctx->hcells_state = 2;
+  CK(cudaMemsetAsync(ctx->d_hcells, 0, ctx->cells * SM_HYDRO_CELL_TERMS * sizeof(double), ctx->stream));
   return SM_OK;
 }
 int sm_water_flood(sm_context* ctx, sm_hydro_stats* st) {
@@ -2235,8 +2284,11 @@ int sm_water_flood(sm_context* ctx, sm_hydro_stats* st) {
   if (rc != SM_OK) return rc;
   if (ctx->cur_kind != KIND_WATER) return fail(ctx, SM_ERR_INVALID, "sm_water_flood: the last batch was not a water batch");
   CK(cudaEventRecord(ctx->ev0, ctx->stream));
-  if (ctx->d.bud) k_hydro_flood_w<true><<<1, 32, 0, ctx->stream>>>(ctx->d, ctx->cur_n, ctx->d_hydro);
-  else if (hydro_warp()) k_hydro_flood_w<false><<<1, 32, 0, ctx->stream>>>(ctx->d, ctx->cur_n, ctx->d_hydro);
+  rc = hydro_cells_reset(ctx);        // inside the call's device time: the maps' whole cost
+  if (rc != SM_OK) return rc;
+  if (ctx->d_hcells) k_hydro_flood_w<true, true><<<1, 32, 0, ctx->stream>>>(ctx->d, ctx->cur_n, ctx->d_hydro, ctx->d_hcells);
+  else if (ctx->d.bud) k_hydro_flood_w<true><<<1, 32, 0, ctx->stream>>>(ctx->d, ctx->cur_n, ctx->d_hydro, nullptr);
+  else if (hydro_warp()) k_hydro_flood_w<false><<<1, 32, 0, ctx->stream>>>(ctx->d, ctx->cur_n, ctx->d_hydro, nullptr);
   else k_hydro_flood<<<1, 32, SM_HC_BYTES, ctx->stream>>>(ctx->d, ctx->cur_n, &ctx->d_hydro->hc);
   ctx->launches++;
   CK(cudaGetLastError());
@@ -2256,12 +2308,15 @@ int sm_seep(sm_context* ctx, sm_hydro_stats* st) {
   unsigned long long off = 0;
   for (int l = 0; l < am.nlevels; l++) { am.lvl[l] = ctx->d_act + off; off += am.nwords[l]; }
   CK(cudaEventRecord(ctx->ev0, ctx->stream));
+  rc = hydro_cells_reset(ctx);        // inside the call's device time: the maps' whole cost
+  if (rc != SM_OK) return rc;
   CK(cudaMemsetAsync(ctx->d_act, 0, total * sizeof(unsigned long long), ctx->stream));
   CK(cudaEventRecord(ctx->evt0, ctx->stream));
   k_hydro_classify<<<ctx->num_sms * 8, 256, 0, ctx->stream>>>(ctx->d, am);
   CK(cudaEventRecord(ctx->evt1, ctx->stream));
-  if (ctx->d.bud) k_hydro_seep_w<true><<<1, 32, 0, ctx->stream>>>(ctx->d, am, ctx->d_hydro);
-  else if (hydro_warp()) k_hydro_seep_w<false><<<1, 32, 0, ctx->stream>>>(ctx->d, am, ctx->d_hydro);
+  if (ctx->d_hcells) k_hydro_seep_w<true, true><<<1, 32, 0, ctx->stream>>>(ctx->d, am, ctx->d_hydro, ctx->d_hcells);
+  else if (ctx->d.bud) k_hydro_seep_w<true><<<1, 32, 0, ctx->stream>>>(ctx->d, am, ctx->d_hydro, nullptr);
+  else if (hydro_warp()) k_hydro_seep_w<false><<<1, 32, 0, ctx->stream>>>(ctx->d, am, ctx->d_hydro, nullptr);
   else k_hydro_seep<<<1, 32, SM_HC_BYTES, ctx->stream>>>(ctx->d, am, &ctx->d_hydro->hc);
   ctx->launches += 2;
   CK(cudaGetLastError());
@@ -2280,6 +2335,26 @@ int sm_last_hydro_budget(sm_context* ctx, sm_hydro_budget* out) {
   out->flood_sediment = b[0]; out->flood_cascade_net = b[1]; out->flood_water = b[2]; out->seeped = b[3];
   out->to_particles = b[4]; out->transfer_net = b[5]; out->nested_eroded = b[6]; out->nested_deposited = b[7];
   out->nested_cascade_net = b[8]; out->nested_discarded = b[9]; out->nested_clamped = b[10];
+  return SM_OK;
+}
+int sm_last_hydro_cell_budget(sm_context* ctx, double* eroded, double* deposited, double* cascade_net, double* water_net) {
+  if (!ctx->d_hcells) return fail(ctx, SM_ERR_INVALID, "context was created without SM_FLAG_HYDRO_CELL_BUDGET");
+  if (ctx->hcells_state == 0) return fail(ctx, SM_ERR_INVALID, "no hydrology call yet (sm_water_flood or sm_seep)");
+  if (ctx->hcells_state == 2)
+    return fail(ctx, SM_ERR_INVALID, "the last hydrology call failed: its per-cell maps are partial");
+  CK(cudaSetDevice(ctx->cfg.device));
+  CK(cudaStreamSynchronize(ctx->stream));
+  // de-interleaved through a bounded host buffer (32 MB), not a host copy of the whole map
+  const size_t chunk = (size_t)1 << 20;
+  std::vector<double> m(std::min(ctx->cells, chunk) * SM_HYDRO_CELL_TERMS);
+  double* const out[SM_HYDRO_CELL_TERMS] = {eroded, deposited, cascade_net, water_net};
+  for (size_t c0 = 0; c0 < ctx->cells; c0 += chunk) {
+    const size_t n = std::min(chunk, ctx->cells - c0);
+    CK(cudaMemcpy(m.data(), ctx->d_hcells + c0 * SM_HYDRO_CELL_TERMS, n * SM_HYDRO_CELL_TERMS * sizeof(double),
+                  cudaMemcpyDeviceToHost));
+    for (int k = 0; k < SM_HYDRO_CELL_TERMS; k++)
+      if (out[k]) for (size_t i = 0; i < n; i++) out[k][c0 + i] = m[i * SM_HYDRO_CELL_TERMS + k];
+  }
   return SM_OK;
 }
 

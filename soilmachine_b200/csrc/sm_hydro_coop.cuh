@@ -31,7 +31,16 @@
 //   6..10                the step budget's slots 0-4 (eroded, deposited, cascade_net, discarded, clamped), summed
 //                        over every step of every nested particle
 // Identity: d(sum of heights) = [0] + [1] + [2] - [3] - [4] + [5] + [7] - [6] + [8], to rounding.
+//
+// Per-cell maps of the same sums (SM_FLAG_HYDRO_CELL_BUDGET): a backing with kCellBudget gets cell_budget(term, x, y,
+// d) at every measurement point above, each delta credited to the cell whose height was read.  Terms 0-2 are the
+// step's (sm_coop.cuh; the nested particles' steps and the flood's terrain cascade call them), plus
+//   1 deposited  the flood's sediment add at the truncated ipos                              (slot 0)
+//   3 water_net  the flood's Air add (+) and every seep(cell) (-, the height removed); a whole water section leaving as
+//                a nested particle at tpos (-); a partial transfer, tpos and bpos each their own change (slots 2-5)
+// Per cell: d(height) = deposited - eroded + cascade_net + water_net, to rounding.
 #define SM_HYDRO_BUDGET_SLOTS 11
+#define SM_HYDRO_CELL_TERMS 4
 
 struct HydroScratch {          // per warp; written by one lane, read by all
   static constexpr bool kBudget = false;
@@ -147,7 +156,7 @@ template <class W, class A, class S> SM_HD void hydro_drain_coop(W& w, A& a, S* 
         if constexpr (S::kBudget) h0 = rec_height(*top);
         a.focus(tx, ty);
         col_remove(a, *top, transfer);
-        if constexpr (S::kBudget) hsx->bud[4] += h0 - rec_height(*top);
+        if constexpr (S::kBudget) { const double d = h0 - rec_height(*top); hsx->bud[4] += d; a.cell_budget(3, tx, ty, -d); }
         a.dirty_rec(top, tx, ty);
       });
       WaterP q;
@@ -193,7 +202,12 @@ template <class W, class A, class S> SM_HD void hydro_drain_coop(W& w, A& a, S* 
         a.focus(bx, by);
         col_add(a, *bot, transfer, SM_AIR);
         if (bot->type != SM_EMPTY) bot->saturation = 1.0;           // map.top(bpos)->saturation = 1.0f
-        if constexpr (S::kBudget) hsx->bud[5] += (rec_height(*top) - ht0) + (rec_height(*bot) - hb0);
+        if constexpr (S::kBudget) {
+          const double dt = rec_height(*top) - ht0, db = rec_height(*bot) - hb0;
+          hsx->bud[5] += dt + db;
+          a.cell_budget(3, tx, ty, dt);
+          a.cell_budget(3, bx, by, db);
+        }
         a.wet_mark(bx, by);
         a.dirty_rec(bot, bx, by);
         if (fspill > 0) fp->spill = fspill - 1;                     // :277-278 cascade(npos, --spill)
@@ -218,7 +232,12 @@ SM_HD void hydro_flood_coop(W& w, A& a, const WaterP& p, int spill, S* hsx, int&
     if constexpr (S::kBudget) h0 = rec_height(*r);
     a.focus(ix, iy);
     col_add(a, *r, sed, what);                                      // :133
-    if constexpr (S::kBudget) { hsx->bud[0] += rec_height(*r) - h0; a.s->acc[2] = 0.0; }   // the cascade sums into acc[2]
+    if constexpr (S::kBudget) {
+      const double d = rec_height(*r) - h0;
+      hsx->bud[0] += d;
+      a.cell_budget(1, ix, iy, d);
+      a.s->acc[2] = 0.0;                                            // the cascade sums into acc[2]
+    }
     a.dirty_rec(r, ix, iy);
   });
   CascadeCoop<0, W, A>::run(w, a, (int)roundf(p.px), (int)roundf(p.py), 0);   // :134
@@ -229,9 +248,14 @@ SM_HD void hydro_flood_coop(W& w, A& a, const WaterP& p, int spill, S* hsx, int&
     a.focus(ix, iy);
     col_add(a, *r, water, SM_AIR);                                  // :138
     a.dirty_rec(r, ix, iy);
-    if constexpr (S::kBudget) { hsx->bud[2] += rec_height(*r) - h0; h0 = rec_height(*r); }
+    if constexpr (S::kBudget) {
+      const double d = rec_height(*r) - h0;
+      hsx->bud[2] += d;
+      a.cell_budget(3, ix, iy, d);
+      h0 = rec_height(*r);
+    }
     hydro_seep_cell(a, ix, iy);                                     // :139
-    if constexpr (S::kBudget) hsx->bud[3] += h0 - rec_height(*r);
+    if constexpr (S::kBudget) { const double d = h0 - rec_height(*r); hsx->bud[3] += d; a.cell_budget(3, ix, iy, -d); }
   });
   hydro_push_coop(w, a, hsx, sp, ix, iy, spill, hc);                // :140
 }
@@ -253,7 +277,7 @@ SM_HD void hydro_seep_visit_coop(W& w, A& a, S* hsx, int x, int y, HydroCount& h
     double h0 = 0.0;
     if constexpr (S::kBudget) h0 = a.height(x, y);
     hydro_seep_cell(a, x, y);
-    if constexpr (S::kBudget) hsx->bud[3] += h0 - a.height(x, y);
+    if constexpr (S::kBudget) { const double d = h0 - a.height(x, y); hsx->bud[3] += d; a.cell_budget(3, x, y, -d); }
   });
   hydro_push_coop(w, a, hsx, sp, x, y, 3, hc);
   hydro_drain_coop(w, a, hsx, sp, hc);
