@@ -100,9 +100,13 @@ int sm_sync(sm_context* ctx);
  * read other ranks' strips, so before calling any of them every rank's earlier work on the map (a batch,
  * sm_initialize, sm_upload_columns) must have completed: sm_sync on every rank, then a host barrier; and no rank may
  * change its strip again until the other ranks' calls have returned (a batch is safe: its ranks meet in a barrier
- * before any of them writes).  The pooling hydrology and the single-cell calls that change the map return
- * SM_ERR_INVALID on a sharded context. */
-#define SM_PEER_ARRAYS 21
+ * before any of them writes).  The pooling hydrology (sm_water_flood, sm_seep) runs on a sharded context from ONE rank,
+ * any rank, that has been named the issuer with sm_hydro_issuer(ctx, 1) and has its peers attached: the call reads and
+ * writes every strip through the peer pointers and the other ranks do not call it; same precondition, and no rank may
+ * touch the map until it returns.  On a rank that is not the issuer these calls return SM_ERR_INVALID, so that a call
+ * made on every rank in lockstep, as the batches are, cannot run several times over the same map.  The single-cell
+ * calls that change the map return SM_ERR_INVALID on a sharded context. */
+#define SM_PEER_ARRAYS 23
 #define SM_PEER_SLOTS 24
 typedef struct sm_peer_blob {
   uint64_t ptr[SM_PEER_SLOTS];
@@ -114,6 +118,10 @@ int sm_create_sharded(const sm_config* cfg, int32_t nranks, int32_t rank, int32_
 int sm_shard_range(sm_context* ctx, int32_t* x0, int32_t* x1);
 int sm_peer_export(sm_context* ctx, sm_peer_blob* out);
 int sm_peer_attach(sm_context* ctx, const sm_peer_blob* blobs, int32_t nblobs, int32_t use_ipc);
+/* on = 1: this rank issues the pooling hydrology of the whole sharded map (sm_water_flood, sm_seep); 0: it does not
+ * (the default).  At most one rank should be the issuer at a time.  No effect on an unsharded context, which always
+ * issues its own. */
+int sm_hydro_issuer(sm_context* ctx, int32_t on);
 
 /* ---- tables: soils[] / layers (surface.h:41-57,104; io.h:7-230 fills them) -------------------- */
 int sm_set_soils(sm_context* ctx, const sm_soil* soils, int32_t n);
@@ -268,10 +276,14 @@ typedef struct sm_hydro_stats {
 } sm_hydro_stats;
 /* WaterParticle::flood (water.h:123-145) for every finished particle of the last water batch, in
  * ascending particle index; each flood is atomic, i.e. the water-table cascade (water.h:151-283) and the
- * particles it spawns run to completion inside it exactly as upstream.  Call after sm_water_run. */
+ * particles it spawns run to completion inside it exactly as upstream.  Call after sm_water_run.
+ * Sharded map: issued from the one rank named by sm_hydro_issuer once every rank's batch has completed (sm_sync on every rank, then a host
+ * barrier); it floods every rank's finished particles over the whole map, bit-identical to one context, on the warp
+ * executor whatever SM_HYDRO says.  Stats, budget and errors belong to the issuing context. */
 int sm_water_flood(sm_context* ctx, sm_hydro_stats* stats);
 /* WaterParticle::seep(map, vertexpool) (water.h:335-343): the per-frame pass over all cells in x-major
- * order, seep(cell) then the water-table cascade with spill 3. */
+ * order, seep(cell) then the water-table cascade with spill 3.  Sharded map: as sm_water_flood (the issuing rank, the
+ * whole map, warp executor). */
 int sm_seep(sm_context* ctx, sm_hydro_stats* stats);
 /* Mass budget of the last successful sm_water_flood or sm_seep call (contexts created with SM_FLAG_BUDGET; such a
  * context runs both on the warp executor whatever SM_HYDRO says).  Same rules as sm_budget: each term is a change
@@ -281,7 +293,8 @@ int sm_seep(sm_context* ctx, sm_hydro_stats* stats);
  * (sm_cell_seep, sm_cell_water_cascade) are not covered.
  * Identity: change of (sum of all column heights) = flood_sediment + flood_cascade_net + flood_water - seeped
  *           - to_particles + transfer_net + nested_deposited - nested_eroded + nested_cascade_net, to rounding.
- * SM_ERR_INVALID without SM_FLAG_BUDGET or before the first hydrology call. */
+ * SM_ERR_INVALID without SM_FLAG_BUDGET or before the first hydrology call.  On a sharded map it reports the last call
+ * THIS context issued (the whole map's budget for that call). */
 typedef struct sm_hydro_budget {
   double flood_sediment;      /* height added by the floods' sediment add                        (water.h:133) */
   double flood_cascade_net;   /* net height change of the floods' terrain cascade, as cascade_net (water.h:134) */
@@ -319,8 +332,8 @@ int sm_last_hydro_budget(sm_context* ctx, sm_hydro_budget* budget);
  * sm_water_flood / sm_seep call inside its device_ms; this call stages the interleaved map through a 32 MB host buffer.
  * SM_ERR_INVALID without SM_FLAG_HYDRO_CELL_BUDGET, before the first sm_water_flood / sm_seep call (a water batch alone
  * does not count), or when the last of these calls failed (its maps were reset and are partial).  sm_create refuses
- * the flag without SM_FLAG_BUDGET, and sm_create_sharded refuses it with nranks > 1: the pooling hydrology does not
- * run on a sharded context. */
+ * the flag without SM_FLAG_BUDGET, and sm_create_sharded refuses it with nranks > 1 (the pooling hydrology runs on a
+ * sharded context without these maps). */
 int sm_last_hydro_cell_budget(sm_context* ctx, double* eroded, double* deposited, double* cascade_net,
                               double* water_net);
 

@@ -36,7 +36,7 @@ SYMBOLS = [
     "sm_wind_sweeps", "sm_wind_state", "sm_launch_count", "sm_device_alloc", "sm_device_free",
     "sm_device_upload", "sm_timer_start", "sm_timer_stop", "sm_set_soil_colors", "sm_mesh_update",
     "sm_mesh_device_ptr", "sm_export_height", "sm_export_color", "sm_create_sharded", "sm_shard_range",
-    "sm_peer_export", "sm_peer_attach", "sm_parse_soil_file", "sm_water_flood", "sm_seep", "sm_last_budget", "sm_budget_particles", "sm_last_cell_budget", "sm_last_hydro_budget", "sm_last_hydro_cell_budget", "sm_lbm_create", "sm_lbm_set_boundary", "sm_lbm_init",
+    "sm_peer_export", "sm_peer_attach", "sm_hydro_issuer", "sm_parse_soil_file", "sm_water_flood", "sm_seep", "sm_last_budget", "sm_budget_particles", "sm_last_cell_budget", "sm_last_hydro_budget", "sm_last_hydro_cell_budget", "sm_lbm_create", "sm_lbm_set_boundary", "sm_lbm_init",
     "sm_lbm_step", "sm_lbm_get", "sm_lbm_advect", "sm_wind_use_lbm",
 ]
 
@@ -183,6 +183,10 @@ class Context:
     def peer_attach(self, blobs, use_ipc):
         arr = (PeerBlob * len(blobs))(*blobs)
         self._ck(self.lib.sm_peer_attach(self.h, arr, len(blobs), int(use_ipc)))
+
+    def hydro_issuer(self, on=True):
+        """sharded map: make this rank the one that issues water_flood / seep for the whole map (or stop it)"""
+        self._ck(self.lib.sm_hydro_issuer(self.h, int(bool(on))))
 
     def close(self):
         if getattr(self, "h", None):

@@ -1172,13 +1172,18 @@ __device__ __forceinline__ void active_set_atomic(const ActiveMap& m, unsigned l
     idx = w;
   }
 }
+// MULTI: the whole map of a sharded context, each column and its buried sections read from the column's owner, into
+// the issuing rank's whole-map bitmap
+template <bool MULTI>
 __global__ void __launch_bounds__(256) k_hydro_classify(DevCtx c, ActiveMap am) {
   const unsigned long long cells = am.ncells;
   for (unsigned long long cell = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; cell < cells;
        cell += (unsigned long long)gridDim.x * blockDim.x) {
-    const Sec32 r = c.top[cell];
+    const Sec32 r = MULTI ? *cell_ptr<MULTI>(c, (int)(cell / (unsigned long long)c.dimy), (int)(cell % (unsigned long long)c.dimy))
+                          : c.top[cell];
     if (r.type == SM_EMPTY) continue;
     const int x = (int)(cell / (unsigned long long)c.dimy), y = (int)(cell % (unsigned long long)c.dimy);
+    const Sec32* const pool = MULTI ? c.peer[owner_of_x<MULTI>(c, x)].pool : c.pool;
     if (r.type == SM_AIR) {
       for (int dx = -1; dx <= 1; dx++) {
         const int xx = x + dx;
@@ -1192,7 +1197,7 @@ __global__ void __launch_bounds__(256) k_hydro_classify(DevCtx c, ActiveMap am) 
     }
     bool holds = (r.saturation != 0.0);
     for (uint32_t b = r.below; !holds && b != SM_NIL;) {
-      const Sec32 s = c.pool[b];
+      const Sec32 s = pool[b];
       holds = (s.saturation != 0.0);
       b = s.below;
     }
@@ -1229,15 +1234,48 @@ template <> struct HydroCellsRef<true> {
   double* hcells;
   __device__ __forceinline__ explicit HydroCellsRef(double* m) : hcells(m) {}
 };
-template <bool BUDGET, bool CELLS = false> struct HydroBack : DevBack<false, BUDGET>, HydroCellsRef<CELLS> {
+// Frequency arrays of every rank of a sharded map.  Rank q's copies are authoritative for the columns of its strip
+// only (the batches write wtrack where the particle is, on the rank that owns that column), so the hydrology reads and
+// writes each cell's words at the column's owner.  A trailing kernel parameter, as CellMaps, so that DevCtx and
+// PeerPtrs keep their layout.
+struct FreqPeers {
+  float* wfreq[SM_MAX_RANKS];
+  float* wtrack[SM_MAX_RANKS];
+};
+template <bool MULTI> struct FreqPeersRef {
+  __device__ __forceinline__ explicit FreqPeersRef(const FreqPeers*) {}
+};
+template <> struct FreqPeersRef<true> {
+  const FreqPeers* fp;
+  __device__ __forceinline__ explicit FreqPeersRef(const FreqPeers* f) : fp(f) {}
+};
+// MULTI: the map is sharded.  Records, pool allocations and frees go to the column's owner (DevBack<true>, steered by
+// the focus() calls of sm_hydro_coop.cuh); the active-cell index is one whole-map bitmap on the issuing rank, indexed
+// by global cell, as on one context.
+template <bool MULTI, bool BUDGET, bool CELLS = false>
+struct HydroBack : DevBack<MULTI, BUDGET>, HydroCellsRef<CELLS>, FreqPeersRef<MULTI> {
   static_assert(!CELLS || BUDGET, "the per-cell maps are measured by the budget instantiations");
+  static_assert(!(CELLS && MULTI), "the hydrology's per-cell maps are not kept on a sharded map");
   static constexpr bool kHydroHooks = true;
   static constexpr bool kCellBudget = CELLS;
   ActiveMap act;
   bool marking;
   __device__ __forceinline__ HydroBack(const DevCtx& ctx, const SoilDev* ss, const ActiveMap& am, bool mk,
-                                       double* cells = nullptr)
-      : DevBack<false, BUDGET>(ctx, ss, 0u), HydroCellsRef<CELLS>(cells), act(am), marking(mk) {}
+                                       double* cells = nullptr, const FreqPeers* fp = nullptr)
+      : DevBack<MULTI, BUDGET>(ctx, ss, 0u), HydroCellsRef<CELLS>(cells), FreqPeersRef<MULTI>(fp), act(am), marking(mk) {}
+  // index i = y*dimx + x
+  __device__ __forceinline__ float wfreq(int i) const {
+    if constexpr (MULTI) return this->fp->wfreq[owner_of_x<true>(this->c, i % this->c.dimx)][i];
+    else return this->c.wfreq[i];
+  }
+  __device__ __forceinline__ float wtrack(int i) const {
+    if constexpr (MULTI) return this->fp->wtrack[owner_of_x<true>(this->c, i % this->c.dimx)][i];
+    else return this->c.wtrack[i];
+  }
+  __device__ __forceinline__ void set_wtrack(int i, float v) {
+    if constexpr (MULTI) this->fp->wtrack[owner_of_x<true>(this->c, i % this->c.dimx)][i] = v;
+    else this->c.wtrack[i] = v;
+  }
   // One fire-and-forget f64 reduction (the rounding of `total += d`), as DevBack::cell_budget: the warp does not wait
   // for it.  One lane of one warp issues them in program order, so each cell's additions land in execution order.  The
   // map is device memory; saying so lets the compiler emit the global-space reduction (ATOMG/RED, no result used)
@@ -1271,9 +1309,15 @@ template <bool BUDGET, class S> __device__ __forceinline__ void hydro_totals_out
   if constexpr (BUDGET)
     for (int k = 0; k < SM_HYDRO_BUDGET_SLOTS; k++) out->bud[k] = hx.bud[k];
 }
-// `hcells`: the per-cell maps with CELLS (HydroBack), a trailing parameter so that DevCtx keeps its layout
-template <bool BUDGET, bool CELLS = false>
-__global__ void __launch_bounds__(32) k_hydro_flood_w(DevCtx c, int n, HydroTotals* out, double* hcells) {
+// `hcells`: the per-cell maps with CELLS (HydroBack), `fp`: the ranks' frequency arrays with MULTI; trailing
+// parameters so that DevCtx keeps its layout.
+// MULTI: the finished particles of a sharded map's last water batch.  A dead particle's final state lives on the rank
+// that ran its last step, and only there does `done` hold the dead marker: every rank clears done[0, n) before a
+// spawning launch (launch_run), and a rank writes a particle's `done` only while it holds the particle.  So the holder
+// is the one rank whose word is 0xFFFFFFFF; the flood reads the state there and leaves SM_DONE_FLOODED there.
+template <bool MULTI, bool BUDGET, bool CELLS = false>
+__global__ void __launch_bounds__(32) k_hydro_flood_w(DevCtx c, int n, HydroTotals* out, double* hcells,
+                                                      const __grid_constant__ FreqPeers fp) {
   __shared__ SoilDev s_soils[SM_MAX_SOILS];
   __shared__ CoopScratch sc;
   __shared__ typename HydroScratchOf<BUDGET>::type hx;
@@ -1283,31 +1327,47 @@ __global__ void __launch_bounds__(32) k_hydro_flood_w(DevCtx c, int n, HydroTota
   __syncwarp();
   WarpDev w{lane};
   ActiveMap none{};
-  HydroBack<BUDGET, CELLS> back(c, s_soils, none, false, hcells);
-  CoopWin<HydroBack<BUDGET, CELLS> > a(back, &sc);
+  HydroBack<MULTI, BUDGET, CELLS> back(c, s_soils, none, false, hcells, &fp);
+  CoopWin<HydroBack<MULTI, BUDGET, CELLS> > a(back, &sc);
   HydroCount hc{};
   for (int base = 0; base < n; base += 32) {
     const int i = base + lane;
     bool cand = false;
-    if (i < n) cand = (c.alive[i] == 0) && !(c.pb[i].x < SM_MINVOL) && c.done[i] != SM_DONE_FLOODED;
+    int holder = 0;
+    if constexpr (MULTI) {
+      if (i < n)
+        for (int q = 0; q < c.nranks; q++)
+          if (c.peer[q].done[i] == 0xFFFFFFFFu) {
+            holder = q;
+            cand = (c.peer[q].alive[i] == 0) && !(c.peer[q].pb[i].x < SM_MINVOL);
+            break;
+          }
+    } else {
+      if (i < n) cand = (c.alive[i] == 0) && !(c.pb[i].x < SM_MINVOL) && c.done[i] != SM_DONE_FLOODED;
+    }
     unsigned int m = __ballot_sync(0xFFFFFFFFu, cand);
     while (m) {                                   // warp-uniform
       const int j = base + __ffs((int)m) - 1;
       m &= m - 1u;
-      const float4 pa = c.pa[j];
-      const double2 pb = c.pb[j];
+      const int q = MULTI ? __shfl_sync(0xFFFFFFFFu, holder, j - base) : 0;
+      const float4 pa = MULTI ? c.peer[q].pa[j] : c.pa[j];
+      const double2 pb = MULTI ? c.peer[q].pb[j] : c.pb[j];
       WaterP p;
       p.px = pa.x; p.py = pa.y; p.sx = pa.z; p.sy = pa.w;
-      p.volume = pb.x; p.sediment = pb.y; p.contains = c.pc[j].x;
+      p.volume = pb.x; p.sediment = pb.y; p.contains = MULTI ? c.peer[q].pc[j].x : c.pc[j].x;
       hydro_flood_particle_coop(w, a, &hx, p, hc);
-      if (lane == 0) c.done[j] = SM_DONE_FLOODED;
+      if (lane == 0) {
+        if (MULTI) c.peer[q].done[j] = SM_DONE_FLOODED;
+        else c.done[j] = SM_DONE_FLOODED;
+      }
       __syncwarp();
     }
   }
   if (lane == 0) hydro_totals_out<BUDGET>(out, hc, hx);
 }
-template <bool BUDGET, bool CELLS = false>
-__global__ void __launch_bounds__(32) k_hydro_seep_w(DevCtx c, ActiveMap am, HydroTotals* out, double* hcells) {
+template <bool MULTI, bool BUDGET, bool CELLS = false>
+__global__ void __launch_bounds__(32) k_hydro_seep_w(DevCtx c, ActiveMap am, HydroTotals* out, double* hcells,
+                                                     const __grid_constant__ FreqPeers fp) {
   __shared__ SoilDev s_soils[SM_MAX_SOILS];
   __shared__ CoopScratch sc;
   __shared__ typename HydroScratchOf<BUDGET>::type hx;
@@ -1316,8 +1376,8 @@ __global__ void __launch_bounds__(32) k_hydro_seep_w(DevCtx c, ActiveMap am, Hyd
   hydro_budget_zero<BUDGET>(hx, lane);
   __syncwarp();
   WarpDev w{lane};
-  HydroBack<BUDGET, CELLS> back(c, s_soils, am, true, hcells);
-  CoopWin<HydroBack<BUDGET, CELLS> > a(back, &sc);
+  HydroBack<MULTI, BUDGET, CELLS> back(c, s_soils, am, true, hcells, &fp);
+  CoopWin<HydroBack<MULTI, BUDGET, CELLS> > a(back, &sc);
   HydroCount hc{};
   const unsigned long long cells = am.ncells;
   for (unsigned long long cell = active_next(am, 0); cell < cells; cell = active_next(am, cell + 1)) {
@@ -1340,6 +1400,7 @@ struct sm_context {
   size_t lcells = 0;       // cells of this rank's x-strip (top records); == cells when not sharded
   int nranks = 1, rank = 0, x0 = 0, x1 = 0, share = 1;
   bool peers_attached = false;
+  bool hydro_issuer = false;      // sharded: this rank issues the pooling hydrology of the whole map (sm_hydro_issuer)
   void* ipc_opened[SM_MAX_RANKS][SM_PEER_SLOTS] = {};
   int max_particles = 0;
   int nsoils = 0;
@@ -1359,7 +1420,8 @@ struct sm_context {
   // per-cell budget maps (SM_FLAG_CELL_BUDGET): 3 f64 per cell of the strip, interleaved; every rank's, by rank
   double* d_cells = nullptr;
   CellMaps cells_of = {};
-  int cells_state = 0;            // 0 no batch yet, 1 the maps cover the last batch, 2 it ran on a kernel without them
+  FreqPeers freq_of = {};         // every rank's frequency arrays, by rank (sharded hydrology)
+  int cells_state = 0;           // 0 no batch yet, 1 the maps cover the last batch, 2 it ran on a kernel without them
   // per-cell maps of the hydrology's budget (SM_FLAG_HYDRO_CELL_BUDGET): SM_HYDRO_CELL_TERMS f64 per cell, interleaved
   double* d_hcells = nullptr;
   int hcells_state = 0;           // 0 no hydrology call yet, 1 the maps cover the last call, 2 that call failed
@@ -1582,6 +1644,7 @@ static void own_ptrs(sm_context* ctx, void** p) {
   p[7] = d.pc; p[8] = d.alive; p[9] = d.done; p[10] = d.head[0]; p[11] = d.head[1]; p[12] = d.node[0]; p[13] = d.node[1];
   p[14] = d.ringbuf[2]; p[15] = d.bud; p[16] = d.fin; p[17] = d.lmask[0]; p[18] = d.lmask[1]; p[19] = d.lmask[2];
   p[20] = ctx->d_cells;
+  p[21] = d.wfreq; p[22] = d.wtrack;    // each its own cudaMalloc (create_impl), as cudaIpcGetMemHandle needs
 }
 static void fill_peer(PeerPtrs& P, void* const* p, unsigned long long pool_cap) {
   P.top = (Sec32*)p[0]; P.pool = (Sec32*)p[1]; P.ringbuf[0] = (uint32_t*)p[2]; P.ringbuf[1] = (uint32_t*)p[3];
@@ -1644,6 +1707,8 @@ int sm_peer_attach(sm_context* ctx, const sm_peer_blob* blobs, int32_t nblobs, i
     }
     fill_peer(ctx->d.peer[q], p, b.pool_cap);
     ctx->cells_of.p[q] = (double*)p[20];
+    ctx->freq_of.wfreq[q] = (float*)p[21];
+    ctx->freq_of.wtrack[q] = (float*)p[22];
   }
   ctx->peers_attached = true;
   return SM_OK;
@@ -1967,6 +2032,11 @@ static int launch_run(sm_context* ctx, int kind, int n, const float* d_spawn, in
   if (multi && !ctx->peers_attached) return fail(ctx, SM_ERR_INVALID, "sharded context: call sm_peer_attach first");
   if (multi && n >= (1 << 28)) return fail(ctx, SM_ERR_INVALID, "sharded context: at most 2^28 particles");
   CK(cudaSetDevice(ctx->cfg.device));
+  // Sharded map, new batch: a rank writes a particle's `done` only while it holds the particle, so without this a
+  // dead marker of an earlier batch would look like the holder's (the flood finds the holder by it, k_hydro_flood_w).
+  // No peer writes into this array before the kernel below has passed its prologue barrier: hand-overs happen in the
+  // sweeps, and that barrier waits for every rank.
+  if (multi && d_spawn != nullptr && n > 0) CK(cudaMemsetAsync(ctx->d.done, 0, (size_t)n * sizeof(unsigned int), ctx->stream));
   const int threads = SM_BLOCK;
   // lanes per particle (a power of two): only the first lane of each group carries a particle, which
   // keeps divergent particle-steps out of each other's warps and shrinks the window footprint
@@ -2222,7 +2292,8 @@ int sm_wind_run_device(sm_context* ctx, int32_t n, const float* d_xy, int32_t ma
 }
 
 // ---- pooling hydrology ----------------------------------------------------------------------------
-// SM_HYDRO=warp | thread selects the executor of the flood phase and the seep pass.  A context created with
+// SM_HYDRO=warp | thread selects the executor of the flood phase and the seep pass.  A sharded context always runs the
+// warp executor (its MULTI instantiations; DESIGN.md section 7).  A context created with
 // SM_FLAG_BUDGET runs the warp executor whatever SM_HYDRO says: the hydrology's budget lives only there, as the
 // batches' budget lives only in the warp sweep kernel.  SM_FLAG_HYDRO_CELL_BUDGET runs its CELLS instantiations.
 static bool hydro_warp() {
@@ -2234,7 +2305,12 @@ static bool hydro_warp() {
 }
 static int hydro_ready(sm_context* ctx) {
   if (ctx->nsoils < 1) return fail(ctx, SM_ERR_INVALID, "soil table not set");
-  if (ctx->nranks > 1) return fail(ctx, SM_ERR_INVALID, "pooling hydrology is not available on a sharded context");
+  // Sharded: the call works on the whole map, so exactly one rank may make it, while the others leave the map alone.
+  // Ranks usually make the same calls in lockstep; a rank only issues the hydrology once it has been named the issuer,
+  // so a symmetric call on every rank is refused instead of running N floods on the same map at once.
+  if (ctx->nranks > 1 && !ctx->hydro_issuer)
+    return fail(ctx, SM_ERR_INVALID, "pooling hydrology is not available on a sharded context that is not the issuing rank (sm_hydro_issuer)");
+  if (ctx->nranks > 1 && !ctx->peers_attached) return fail(ctx, SM_ERR_INVALID, "sharded context: call sm_peer_attach first");
   CK(cudaSetDevice(ctx->cfg.device));
   if (!ctx->d_hydro) {
     CK(cudaMalloc(&ctx->d_hydro, sizeof(HydroTotals)));
@@ -2279,6 +2355,10 @@ static int hydro_cells_reset(sm_context* ctx) {
   CK(cudaMemsetAsync(ctx->d_hcells, 0, ctx->cells * SM_HYDRO_CELL_TERMS * sizeof(double), ctx->stream));
   return SM_OK;
 }
+int sm_hydro_issuer(sm_context* ctx, int32_t on) {
+  ctx->hydro_issuer = on != 0;
+  return SM_OK;
+}
 int sm_water_flood(sm_context* ctx, sm_hydro_stats* st) {
   int rc = hydro_ready(ctx);
   if (rc != SM_OK) return rc;
@@ -2286,9 +2366,14 @@ int sm_water_flood(sm_context* ctx, sm_hydro_stats* st) {
   CK(cudaEventRecord(ctx->ev0, ctx->stream));
   rc = hydro_cells_reset(ctx);        // inside the call's device time: the maps' whole cost
   if (rc != SM_OK) return rc;
-  if (ctx->d_hcells) k_hydro_flood_w<true, true><<<1, 32, 0, ctx->stream>>>(ctx->d, ctx->cur_n, ctx->d_hydro, ctx->d_hcells);
-  else if (ctx->d.bud) k_hydro_flood_w<true><<<1, 32, 0, ctx->stream>>>(ctx->d, ctx->cur_n, ctx->d_hydro, nullptr);
-  else if (hydro_warp()) k_hydro_flood_w<false><<<1, 32, 0, ctx->stream>>>(ctx->d, ctx->cur_n, ctx->d_hydro, nullptr);
+  const FreqPeers& fp = ctx->freq_of;
+  if (ctx->nranks > 1) {     // sharded: the warp executor, whatever SM_HYDRO says
+    if (ctx->d.bud) k_hydro_flood_w<true, true><<<1, 32, 0, ctx->stream>>>(ctx->d, ctx->cur_n, ctx->d_hydro, nullptr, fp);
+    else k_hydro_flood_w<true, false><<<1, 32, 0, ctx->stream>>>(ctx->d, ctx->cur_n, ctx->d_hydro, nullptr, fp);
+  }
+  else if (ctx->d_hcells) k_hydro_flood_w<false, true, true><<<1, 32, 0, ctx->stream>>>(ctx->d, ctx->cur_n, ctx->d_hydro, ctx->d_hcells, fp);
+  else if (ctx->d.bud) k_hydro_flood_w<false, true><<<1, 32, 0, ctx->stream>>>(ctx->d, ctx->cur_n, ctx->d_hydro, nullptr, fp);
+  else if (hydro_warp()) k_hydro_flood_w<false, false><<<1, 32, 0, ctx->stream>>>(ctx->d, ctx->cur_n, ctx->d_hydro, nullptr, fp);
   else k_hydro_flood<<<1, 32, SM_HC_BYTES, ctx->stream>>>(ctx->d, ctx->cur_n, &ctx->d_hydro->hc);
   ctx->launches++;
   CK(cudaGetLastError());
@@ -2312,12 +2397,20 @@ int sm_seep(sm_context* ctx, sm_hydro_stats* st) {
   if (rc != SM_OK) return rc;
   CK(cudaMemsetAsync(ctx->d_act, 0, total * sizeof(unsigned long long), ctx->stream));
   CK(cudaEventRecord(ctx->evt0, ctx->stream));
-  k_hydro_classify<<<ctx->num_sms * 8, 256, 0, ctx->stream>>>(ctx->d, am);
-  CK(cudaEventRecord(ctx->evt1, ctx->stream));
-  if (ctx->d_hcells) k_hydro_seep_w<true, true><<<1, 32, 0, ctx->stream>>>(ctx->d, am, ctx->d_hydro, ctx->d_hcells);
-  else if (ctx->d.bud) k_hydro_seep_w<true><<<1, 32, 0, ctx->stream>>>(ctx->d, am, ctx->d_hydro, nullptr);
-  else if (hydro_warp()) k_hydro_seep_w<false><<<1, 32, 0, ctx->stream>>>(ctx->d, am, ctx->d_hydro, nullptr);
-  else k_hydro_seep<<<1, 32, SM_HC_BYTES, ctx->stream>>>(ctx->d, am, &ctx->d_hydro->hc);
+  const FreqPeers& fp = ctx->freq_of;
+  if (ctx->nranks > 1) {     // sharded: the whole map, each column read at its owner; then the warp executor
+    k_hydro_classify<true><<<ctx->num_sms * 8, 256, 0, ctx->stream>>>(ctx->d, am);
+    CK(cudaEventRecord(ctx->evt1, ctx->stream));
+    if (ctx->d.bud) k_hydro_seep_w<true, true><<<1, 32, 0, ctx->stream>>>(ctx->d, am, ctx->d_hydro, nullptr, fp);
+    else k_hydro_seep_w<true, false><<<1, 32, 0, ctx->stream>>>(ctx->d, am, ctx->d_hydro, nullptr, fp);
+  } else {
+    k_hydro_classify<false><<<ctx->num_sms * 8, 256, 0, ctx->stream>>>(ctx->d, am);
+    CK(cudaEventRecord(ctx->evt1, ctx->stream));
+    if (ctx->d_hcells) k_hydro_seep_w<false, true, true><<<1, 32, 0, ctx->stream>>>(ctx->d, am, ctx->d_hydro, ctx->d_hcells, fp);
+    else if (ctx->d.bud) k_hydro_seep_w<false, true><<<1, 32, 0, ctx->stream>>>(ctx->d, am, ctx->d_hydro, nullptr, fp);
+    else if (hydro_warp()) k_hydro_seep_w<false, false><<<1, 32, 0, ctx->stream>>>(ctx->d, am, ctx->d_hydro, nullptr, fp);
+    else k_hydro_seep<<<1, 32, SM_HC_BYTES, ctx->stream>>>(ctx->d, am, &ctx->d_hydro->hc);
+  }
   ctx->launches += 2;
   CK(cudaGetLastError());
   int rc2 = hydro_finish(ctx, st);

@@ -120,6 +120,24 @@ class VirtualShards:
         parts = [c.last_cell_budget() for c in self.ctx]
         return {k: np.concatenate([p[k] for p in parts], axis=0) for k in capi.CELL_TERMS}
 
+    # ---- pooling hydrology: one rank issues the call, which reads and writes every strip ----
+    def _hydro(self, rank, call):
+        self.sync()
+        for r, c in enumerate(self.ctx):          # ctx[rank] is the only issuer
+            c.hydro_issuer(r == rank)
+        st = call(self.ctx[rank])
+        self.sync()
+        return st
+
+    def water_flood(self, rank=0):
+        """flood() of every finished particle of the last water batch over the whole map, issued by ctx[rank]; the
+        stats, the budget (ctx[rank].last_hydro_budget()) and any error belong to that context"""
+        return self._hydro(rank, lambda c: c.water_flood())
+
+    def seep(self, rank=0):
+        """the seep pass over the whole map, issued by ctx[rank]"""
+        return self._hydro(rank, lambda c: c.seep())
+
     # ---- read-only views of the whole map (meshing, export, queries, wind-field boundary) ----
     # Each of these reads other ranks' strips, so every rank's earlier work must have completed first: sync() does
     # that for contexts of this process.
@@ -209,6 +227,24 @@ class DistShard:
         ranks' steps write into this strip, so every rank's batch has to be complete first)"""
         self._settle()
         return self.ctx.last_cell_budget()
+
+    # ---- pooling hydrology: every process calls, the issuer's context runs it over the whole map ----
+    def water_flood(self, issuer=0):
+        """flood() of every finished particle of the last water batch; all ranks must call it.  Returns the stats on
+        the issuer and None elsewhere (the issuer's context also holds the budget and any error)."""
+        self._settle()
+        self.ctx.hydro_issuer(self.rank == issuer)
+        st = self.ctx.water_flood() if self.rank == issuer else None
+        self.dist.barrier()
+        return st
+
+    def seep(self, issuer=0):
+        """the seep pass over the whole map; all ranks must call it.  Stats on the issuer, None elsewhere."""
+        self._settle()
+        self.ctx.hydro_issuer(self.rank == issuer)
+        st = self.ctx.seep() if self.rank == issuer else None
+        self.dist.barrier()
+        return st
 
     # ---- read-only views of the whole map ----
     # The calls that read other ranks' strips first wait for this rank's work and then meet every other rank in a
