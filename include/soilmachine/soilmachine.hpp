@@ -139,8 +139,14 @@ class Layermap {
   ivec2 dim; secpool pool; unsigned* section = nullptr;
   sm_context* ctx = nullptr;
 
-  Layermap(int SEED, ivec2 _dim, int SCALE = 80, int device = 0) { pool.reserve(256); open(_dim, SCALE, device); initialize(SEED, _dim); }
-  template <class VP> Layermap(int SEED, ivec2 _dim, VP&, int SCALE = 80, int device = 0) : Layermap(SEED, _dim, SCALE, device) {}
+  // Several GPUs: ngpus > 1 cuts the map into that many x-strips, rank r on devices[r] (default device + r); every
+  // call below then acts on the whole map exactly as on one GPU (sm_create_group).  ngpus = 0 reads the environment:
+  // SM_GPUS=N, and SM_GPU_DEVICES=0,0 for a device list (equal entries: ranks sharing a GPU).  0 or 1: one context.
+  Layermap(int SEED, ivec2 _dim, int SCALE = 80, int device = 0, int ngpus = 0, const int* devices = nullptr) {
+    pool.reserve(256); open(_dim, SCALE, device, ngpus, devices); initialize(SEED, _dim);
+  }
+  template <class VP> Layermap(int SEED, ivec2 _dim, VP&, int SCALE = 80, int device = 0, int ngpus = 0,
+                               const int* devices = nullptr) : Layermap(SEED, _dim, SCALE, device, ngpus, devices) {}
   ~Layermap() { if (ctx) sm_destroy(ctx); }
   Layermap(const Layermap&) = delete;
 
@@ -264,10 +270,32 @@ class Layermap {
     vp.upload(vertices.data(), (size_t)dim.x * dim.y);
   }
   template <class VP> void upload_if_possible(VP&, long) {}
-  void open(ivec2 _dim, int SCALE, int device) {
+  void open(ivec2 _dim, int SCALE, int device, int ngpus = 0, const int* devices = nullptr) {
     dim = _dim;
     sm_config cfg{dim.x, dim.y, SCALE, device, 0, 0, 0};
-    int rc = sm_create(&cfg, &ctx);
+    std::vector<int32_t> devs;
+    if (ngpus <= 0) {
+      const char* e = std::getenv("SM_GPUS");
+      ngpus = e ? std::atoi(e) : 1;
+      if (const char* l = std::getenv("SM_GPU_DEVICES"))
+        for (const char* q = l; *q;) {
+          char* end = nullptr;
+          const long v = std::strtol(q, &end, 10);
+          if (end == q) break;
+          devs.push_back((int32_t)v);
+          q = (*end == ',') ? end + 1 : end;
+        }
+    } else if (devices) {
+      devs.assign(devices, devices + ngpus);
+    }
+    int rc;
+    if (ngpus <= 1) {
+      rc = sm_create(&cfg, &ctx);
+    } else {
+      if (devs.empty()) for (int r = 0; r < ngpus; r++) devs.push_back(device + r);
+      if ((int)devs.size() != ngpus) throw Error(SM_ERR_INVALID, "Layermap: one device per GPU rank (SM_GPU_DEVICES)");
+      rc = sm_create_group(&cfg, ngpus, devs.data(), &ctx);
+    }
     if (rc != SM_OK) throw Error(rc, sm_last_error(nullptr));
   }
 };

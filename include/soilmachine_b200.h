@@ -105,7 +105,8 @@ int sm_sync(sm_context* ctx);
  * writes every strip through the peer pointers and the other ranks do not call it; same precondition, and no rank may
  * touch the map until it returns.  On a rank that is not the issuer these calls return SM_ERR_INVALID, so that a call
  * made on every rank in lockstep, as the batches are, cannot run several times over the same map.  The single-cell
- * calls that change the map return SM_ERR_INVALID on a sharded context. */
+ * calls that change the map return SM_ERR_INVALID on a sharded context; a group (sm_create_group) offers them.
+ * sm_peer_attach with use_ipc = 0 enables peer access to a blob's device when it differs from the context's. */
 #define SM_PEER_ARRAYS 23
 #define SM_PEER_SLOTS 24
 typedef struct sm_peer_blob {
@@ -122,6 +123,47 @@ int sm_peer_attach(sm_context* ctx, const sm_peer_blob* blobs, int32_t nblobs, i
  * (the default).  At most one rank should be the issuer at a time.  No effect on an unsharded context, which always
  * issues its own. */
 int sm_hydro_issuer(sm_context* ctx, int32_t on);
+
+/* ---- groups: a sharded map behind ONE context (every rank in this process) ----------------------------- */
+/* One handle over a map cut into nranks x-strips, all ranks living in THIS process.  devices[r] = CUDA ordinal of
+ * rank r; devices == NULL: every rank on cfg->device.  Ranks with equal entries share that device (each is created
+ * with share = ranks on that device).  nranks == 1 behaves exactly as sm_create (on devices[0] if given).
+ * The group creates one sm_create_sharded context per rank, attaches them to each other without IPC (enabling peer
+ * access between different devices; SM_ERR_CUDA "no peer access between devices a and b" where the hardware has none)
+ * and issues the pooling hydrology from rank 0.  Every sm_* call that takes a context takes the group and acts on the
+ * WHOLE map in the unsharded cell order (x*dimy + y; frequency arrays y*dimx + x): callers never see strips, and the
+ * results are bit-identical to one context.  What the calls do on a group:
+ *   tables, sm_initialize, sm_frequency_update, sm_lbm_create/_set_boundary/_init/_step, sm_wind_use_lbm, sm_sync:
+ *     every rank (sm_lbm_step reports the slowest rank's time);
+ *   sm_upload_columns, sm_set_frequency: the whole-map input is cut at the strips;
+ *   downloads, sm_mesh_update (host vertices), sm_export_*, sm_last_cell_budget: each rank writes its slice of the
+ *     caller's whole-map buffer; sm_checksum adds the ranks' checksums; sm_height_sum runs the one-context reduction
+ *     tree over the whole map from rank 0;
+ *   batches (sm_*_run, *_run_device, *_begin, *_sweeps): the spawn list goes to every rank and every rank's kernel is
+ *     launched before anything waits for one (they meet in a cross-rank barrier each sweep).  For *_run_device the list
+ *     lives on rank 0's device (sm_device_* act on rank 0) and is copied to the other ranks asynchronously.  Stats:
+ *     steps, exits and pool_drops are summed; sweeps, alive and device_ms are the largest rank's.  sm_last_budget sums
+ *     the ranks per particle, then in particle order; sm_*_state takes each particle from the rank that holds it;
+ *   sm_water_flood, sm_seep, sm_last_hydro_budget, sm_cell_query, sm_height_bilinear, sm_cell_column, sm_lbm_get,
+ *     sm_lbm_advect, sm_timer_*, sm_device_*: rank 0 (the first six after every rank's work has completed);
+ *   sm_cell_add / _remove / _cascade / _seep / _water_cascade: one warp on rank 0 that sends every record access, pool
+ *     allocation and free to the column's owner;
+ *   sm_launch_count: the ranks' launches summed; sm_last_error: the failing rank's message, prefixed "rank r: ";
+ *   sm_mesh_device_ptr: SM_ERR_INVALID (there is no single device array: sm_group_rank + the rank's pointer);
+ *   sm_peer_export, sm_peer_attach, sm_hydro_issuer: SM_ERR_INVALID (the group manages its ranks).
+ * The group waits for every rank (sm_sync on each) before a call that reads or writes other ranks' strips, and only
+ * when something was enqueued since the last wait.  SM_FLAG_BUDGET and SM_FLAG_CELL_BUDGET pass through to the ranks;
+ * SM_FLAG_HYDRO_CELL_BUDGET with nranks > 1 is refused as by sm_create_sharded.  pool_capacity == 0 keeps the sharded
+ * auto rule; a non-zero value is the WHOLE map's capacity, divided among the ranks by strip cells, rounded up.
+ * sm_destroy waits for every rank, batches still in flight included, before it frees anything. */
+int sm_create_group(const sm_config* cfg, int32_t nranks, const int32_t* devices, sm_context** out);
+/* the rank contexts, for tests and tools (owned by the group; do not destroy) */
+int sm_group_size(sm_context* ctx, int32_t* nranks);           /* 1 for a plain context */
+int sm_group_rank(sm_context* ctx, int32_t rank, sm_context** rank_ctx);
+/* Host only, no device needed: the strip [x0, x1) sm_create_group / sm_create_sharded give rank `rank` of nranks, and
+ * the pool_capacity a group hands that rank (0 = auto).  SM_ERR_INVALID, with sm_create_sharded's message in
+ * sm_last_error(NULL), when the map is too narrow for that many ranks.  Any out pointer may be NULL. */
+int sm_group_layout(const sm_config* cfg, int32_t nranks, int32_t rank, int32_t* x0, int32_t* x1, int64_t* pool_capacity);
 
 /* ---- tables: soils[] / layers (surface.h:41-57,104; io.h:7-230 fills them) -------------------- */
 int sm_set_soils(sm_context* ctx, const sm_soil* soils, int32_t n);
@@ -170,7 +212,7 @@ int sm_set_soil_colors(sm_context* ctx, const float* rgba, int32_t n);
  * SLICE (SoilMachine.cpp:12).  The vertices stay in device memory (sm_mesh_device_ptr, e.g. for GL
  * interop); host_vertices may be NULL or a buffer of cells*11 floats (cells of this rank's strip on a sharded map). */
 int sm_mesh_update(sm_context* ctx, int32_t slice, float* host_vertices);
-int sm_mesh_device_ptr(sm_context* ctx, void** dptr);
+int sm_mesh_device_ptr(sm_context* ctx, void** dptr);   /* SM_ERR_INVALID on a group of several ranks */
 /* exportheight / exportcolor (io.h:234-252): the values the reference writes to the PNGs, as floats:
  * height[cell] = position.y / SCALE / sqrt(2); color[cell*4..] = (b, g, r, 1) of the vertex colour.
  * Both read the mesh of the last sm_mesh_update. */

@@ -38,6 +38,7 @@ SYMBOLS = [
     "sm_mesh_device_ptr", "sm_export_height", "sm_export_color", "sm_create_sharded", "sm_shard_range",
     "sm_peer_export", "sm_peer_attach", "sm_hydro_issuer", "sm_parse_soil_file", "sm_water_flood", "sm_seep", "sm_last_budget", "sm_budget_particles", "sm_last_cell_budget", "sm_last_hydro_budget", "sm_last_hydro_cell_budget", "sm_lbm_create", "sm_lbm_set_boundary", "sm_lbm_init",
     "sm_lbm_step", "sm_lbm_get", "sm_lbm_advect", "sm_wind_use_lbm",
+    "sm_create_group", "sm_group_size", "sm_group_rank", "sm_group_layout",
 ]
 
 
@@ -147,12 +148,16 @@ class PeerBlob(C.Structure):
 
 
 class Context:
-    """One sm_context (one GPU, or one rank of a sharded map)."""
+    """One sm_context: one GPU, one rank of a sharded map, or (gpus > 1) a group over a map sharded in this process."""
 
     def __init__(self, dimx, dimy, scale=80, device=0, pool_capacity=0, max_particles=0,
-                 nranks=1, rank=0, share=1, budget=False, cell_budget=False, hydro_cell_budget=False):
+                 nranks=1, rank=0, share=1, budget=False, cell_budget=False, hydro_cell_budget=False,
+                 gpus=1, devices=None):
         """cell_budget=True keeps the per-cell budget maps of the batches as well (SM_FLAG_BUDGET | SM_FLAG_CELL_BUDGET),
-        hydro_cell_budget=True those of the hydrology calls (SM_FLAG_BUDGET | SM_FLAG_HYDRO_CELL_BUDGET)"""
+        hydro_cell_budget=True those of the hydrology calls (SM_FLAG_BUDGET | SM_FLAG_HYDRO_CELL_BUDGET).
+        gpus=N (or devices=[ordinal of rank 0, ...]) creates the context with sm_create_group: the map is cut into N
+        x-strips, one rank per entry of `devices` (default: device, device + 1, ...; equal entries share a GPU), and
+        every method below acts on the whole map exactly as on one context."""
         self.lib = load()
         self.dimx, self.dimy, self.scale = int(dimx), int(dimy), int(scale)
         flags = 3 if cell_budget else (1 if budget else 0)     # SM_FLAG_BUDGET | SM_FLAG_CELL_BUDGET
@@ -160,7 +165,13 @@ class Context:
             flags |= 1 | 4                                     # SM_FLAG_BUDGET | SM_FLAG_HYDRO_CELL_BUDGET
         cfg = Config(self.dimx, self.dimy, self.scale, int(device), int(pool_capacity), int(max_particles), flags)
         h = C.c_void_p()
-        if nranks == 1:
+        if devices is not None:
+            gpus = len(devices)
+        if gpus > 1 or devices is not None:
+            assert nranks == 1, "a group creates its own ranks"
+            devs = (C.c_int32 * gpus)(*(devices if devices is not None else range(int(device), int(device) + gpus)))
+            rc = self.lib.sm_create_group(C.byref(cfg), int(gpus), devs, C.byref(h))
+        elif nranks == 1:
             rc = self.lib.sm_create(C.byref(cfg), C.byref(h))
         else:
             rc = self.lib.sm_create_sharded(C.byref(cfg), int(nranks), int(rank), int(share), C.byref(h))
@@ -174,6 +185,17 @@ class Context:
         self.map_cells = self.dimx * self.dimy                 # whole map (frequency arrays)
         self.cells = (self.x1 - self.x0) * self.dimy           # this rank's strip (columns, heights)
         self._n = {"water": 0, "wind": 0}
+
+    def group_size(self):
+        n = C.c_int32()
+        self._ck(self.lib.sm_group_size(self.h, C.byref(n)))
+        return n.value
+
+    def group_rank(self, rank):
+        """the raw handle of rank `rank` of a group (owned by the group), for tests and tools"""
+        h = C.c_void_p()
+        self._ck(self.lib.sm_group_rank(self.h, int(rank), C.byref(h)))
+        return h
 
     def peer_export(self):
         b = PeerBlob()

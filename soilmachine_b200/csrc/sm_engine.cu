@@ -784,12 +784,16 @@ __global__ void k_heights(const Sec32* __restrict__ top, double* __restrict__ ou
 
 // deterministic sum: fixed chunking, fixed in-block tree; second pass sums the partials in order
 #define SUM_BLOCKS 1024
-__global__ void k_height_sum1(const Sec32* __restrict__ top, size_t n, double* __restrict__ partial) {
+// MULTI: the n cells of the whole sharded map in global cell order, each read from its column's owner, so that the
+// tree - and with it every bit of the sum - is the one context's
+template <bool MULTI> __global__ void k_height_sum1(DevCtx c, size_t n, double* __restrict__ partial) {
+  const Sec32* __restrict__ const top = c.top;
   __shared__ double sh[256];
   const size_t chunk = (n + SUM_BLOCKS - 1) / SUM_BLOCKS;
   const size_t lo = (size_t)blockIdx.x * chunk, hi = (lo + chunk < n) ? lo + chunk : n;
   double acc = 0.0;
-  for (size_t i = lo + threadIdx.x; i < hi; i += 256) acc += rec_height(top[i]);
+  for (size_t i = lo + threadIdx.x; i < hi; i += 256)
+    acc += rec_height(MULTI ? *cell_ptr<MULTI>(c, (int)(i / (size_t)c.dimy), (int)(i % (size_t)c.dimy)) : top[i]);
   sh[threadIdx.x] = acc;
   __syncthreads();
   for (int s2 = 128; s2 > 0; s2 >>= 1) {
@@ -1390,7 +1394,9 @@ __global__ void __launch_bounds__(32) k_hydro_seep_w(DevCtx c, ActiveMap am, Hyd
 // ---------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------
+struct sm_group;
 struct sm_context {
+  sm_group* group = nullptr;      // set: this context is a group of rank contexts (sm_create_group, sm_group.cuh)
   sm_config cfg;
   DevCtx d;
   std::string err;
@@ -1458,12 +1464,15 @@ static void host_soil_to_dev(const sm_soil& s, SoilDev& d) {
   d.cascades = (uint32_t)s.cascades; d.abrades = (uint32_t)s.abrades;
 }
 
+#include "sm_group.cuh"
+
 extern "C" {
 
 const char* sm_last_error(const sm_context* ctx) { return ctx ? ctx->err.c_str() : g_create_err.c_str(); }
 
 void sm_destroy(sm_context* ctx) {
   if (!ctx) return;
+  if (ctx->group) { grp_destroy(ctx); return; }
   cudaSetDevice(ctx->cfg.device);
   cudaDeviceSynchronize();
   for (int q = 0; q < SM_MAX_RANKS; q++) for (int i = 0; i < SM_PEER_SLOTS; i++) if (ctx->ipc_opened[q][i]) cudaIpcCloseMemHandle(ctx->ipc_opened[q][i]);
@@ -1519,11 +1528,9 @@ static int create_impl(const sm_config* cfg, int nranks, int rank, int share, sm
                    "sharded context";
     return SM_ERR_INVALID;
   }
-  // x-strips of equal width (a multiple of the largest bin edge, 16 cells)
-  const int strip_w = (nranks == 1) ? cfg->dimx : ((((cfg->dimx + nranks - 1) / nranks) + 15) / 16) * 16;
-  const int sx0 = rank * strip_w, sx1 = std::min(cfg->dimx, sx0 + strip_w);
-  if (sx1 <= sx0) {
-    g_create_err = "sm_create_sharded: the map is too narrow for this many ranks (needs >= 16 columns per rank)";
+  int strip_w, sx0, sx1;
+  if (!shard_strip(cfg->dimx, nranks, rank, &strip_w, &sx0, &sx1)) {
+    g_create_err = kStripTooNarrow;
     return SM_ERR_INVALID;
   }
   int ndev = 0;
@@ -1631,6 +1638,35 @@ int sm_create(const sm_config* cfg, sm_context** out) { return create_impl(cfg, 
 int sm_create_sharded(const sm_config* cfg, int32_t nranks, int32_t rank, int32_t share, sm_context** out) {
   return create_impl(cfg, nranks, rank, share, out);
 }
+int sm_create_group(const sm_config* cfg, int32_t nranks, const int32_t* devices, sm_context** out) {
+  return grp_create(cfg, nranks, devices, out);
+}
+int sm_group_size(sm_context* ctx, int32_t* nranks) {
+  if (!nranks) return fail(ctx, SM_ERR_INVALID, "null argument");
+  *nranks = ctx->group ? ctx->group->n : 1;
+  return SM_OK;
+}
+int sm_group_rank(sm_context* ctx, int32_t rank, sm_context** rank_ctx) {
+  const int n = ctx->group ? ctx->group->n : 1;
+  if (!rank_ctx || rank < 0 || rank >= n) return fail(ctx, SM_ERR_INVALID, "sm_group_rank: rank out of range");
+  *rank_ctx = ctx->group ? ctx->group->rank[rank] : ctx;
+  return SM_OK;
+}
+int sm_group_layout(const sm_config* cfg, int32_t nranks, int32_t rank, int32_t* x0, int32_t* x1, int64_t* pool_capacity) {
+  int w, a, b;
+  if (!cfg || nranks < 1 || nranks > SM_MAX_RANKS || rank < 0 || rank >= nranks || cfg->dimx < 2) {
+    g_create_err = "sm_group_layout: invalid arguments";
+    return SM_ERR_INVALID;
+  }
+  if (!shard_strip(cfg->dimx, nranks, rank, &w, &a, &b)) {
+    g_create_err = kStripTooNarrow;
+    return SM_ERR_INVALID;
+  }
+  if (x0) *x0 = a;
+  if (x1) *x1 = b;
+  if (pool_capacity) *pool_capacity = nranks == 1 ? cfg->pool_capacity : shard_pool_capacity(cfg->pool_capacity, cfg->dimx, a, b);
+  return SM_OK;
+}
 int sm_shard_range(sm_context* ctx, int32_t* x0, int32_t* x1) {
   if (x0) *x0 = ctx->x0;
   if (x1) *x1 = ctx->x1;
@@ -1656,6 +1692,7 @@ static void fill_peer(PeerPtrs& P, void* const* p, unsigned long long pool_cap) 
   P.pool_cap = pool_cap;
 }
 int sm_peer_export(sm_context* ctx, sm_peer_blob* out) {
+  if (ctx->group) return fail(ctx, SM_ERR_INVALID, "a group manages its ranks' peers itself (sm_group_rank gives the rank contexts)");
   if (!out) return fail(ctx, SM_ERR_INVALID, "null blob");
   CK(cudaSetDevice(ctx->cfg.device));
   memset(out, 0, sizeof(*out));
@@ -1675,6 +1712,7 @@ int sm_peer_export(sm_context* ctx, sm_peer_blob* out) {
   return SM_OK;
 }
 int sm_peer_attach(sm_context* ctx, const sm_peer_blob* blobs, int32_t nblobs, int32_t use_ipc) {
+  if (ctx->group) return fail(ctx, SM_ERR_INVALID, "a group manages its ranks' peers itself (sm_group_rank gives the rank contexts)");
   if (!blobs || nblobs != ctx->nranks) return fail(ctx, SM_ERR_INVALID, "sm_peer_attach: one blob per rank");
   for (int q = 0; q < nblobs; q++)   // slot 20: the per-cell budget maps; a step writes into its neighbours' maps
     if ((blobs[q].ptr[20] != 0) != (ctx->d_cells != nullptr))
@@ -1684,19 +1722,25 @@ int sm_peer_attach(sm_context* ctx, const sm_peer_blob* blobs, int32_t nblobs, i
     const sm_peer_blob& b = blobs[q];
     if (b.rank != q) return fail(ctx, SM_ERR_INVALID, "sm_peer_attach: blobs must be ordered by rank");
     void* p[SM_PEER_SLOTS] = {};
+    if (q != ctx->rank && b.device != ctx->cfg.device) {
+      // this rank's kernels dereference the peer's pointers: raw ones of the same process need the access enabled just
+      // as IPC mappings do (every rank attaches every other, so both directions get enabled)
+      int can = 0;
+      CK(cudaDeviceCanAccessPeer(&can, ctx->cfg.device, b.device));
+      if (!can) {
+        ctx->err = "sm_peer_attach: no peer access between devices " + std::to_string(ctx->cfg.device) + " and " +
+                   std::to_string(b.device);
+        return SM_ERR_CUDA;
+      }
+      cudaError_t e = cudaDeviceEnablePeerAccess(b.device, 0);
+      if (e != cudaSuccess && e != cudaErrorPeerAccessAlreadyEnabled) { ctx->err = cudaGetErrorString(e); return SM_ERR_CUDA; }
+      cudaGetLastError();      // cudaErrorPeerAccessAlreadyEnabled is sticky until read
+    }
     if (q == ctx->rank) {
       own_ptrs(ctx, p);
     } else if (!use_ipc) {
       for (int i = 0; i < SM_PEER_ARRAYS; i++) p[i] = (void*)(uintptr_t)b.ptr[i];   // same process
     } else {
-      if (b.device != ctx->cfg.device) {
-        int can = 0;
-        CK(cudaDeviceCanAccessPeer(&can, ctx->cfg.device, b.device));
-        if (!can) return fail(ctx, SM_ERR_CUDA, "sm_peer_attach: no peer access between the devices");
-        cudaError_t e = cudaDeviceEnablePeerAccess(b.device, 0);
-        if (e != cudaSuccess && e != cudaErrorPeerAccessAlreadyEnabled) { ctx->err = cudaGetErrorString(e); return SM_ERR_CUDA; }
-        cudaGetLastError();
-      }
       for (int i = 0; i < SM_PEER_ARRAYS; i++) {
         if (!b.ptr[i]) continue;
         cudaIpcMemHandle_t h;
@@ -1715,12 +1759,18 @@ int sm_peer_attach(sm_context* ctx, const sm_peer_blob* blobs, int32_t nblobs, i
 }
 
 int sm_sync(sm_context* ctx) {
+  if (ctx->group) return grp_settle(ctx);
   CK(cudaSetDevice(ctx->cfg.device));
   CK(cudaStreamSynchronize(ctx->stream));
   return SM_OK;
 }
 
 int sm_set_soils(sm_context* ctx, const sm_soil* soils, int32_t n) {
+  if (ctx->group) {
+    const int rc = grp_each(ctx, [&](sm_context* c, int) { return sm_set_soils(c, soils, n); });
+    if (rc == SM_OK) ctx->nsoils = n;
+    return rc;
+  }
   if (!soils || n < 1 || n > SM_MAX_SOILS) return fail(ctx, SM_ERR_INVALID, "sm_set_soils: 1..64 soils");
   for (int i = 0; i < n; i++) {
     const sm_soil& s = soils[i];
@@ -1765,6 +1815,7 @@ static int reset_pool_ctl(sm_context* ctx, unsigned long long used) {
 
 int sm_upload_columns(sm_context* ctx, const int64_t* offsets, const int32_t* type, const double* size,
                       const double* saturation) {
+  if (ctx->group) return grp_upload_columns(ctx, offsets, type, size, saturation);
   if (!offsets || !type || !size) return fail(ctx, SM_ERR_INVALID, "sm_upload_columns: null argument");
   CK(cudaSetDevice(ctx->cfg.device));
   const size_t C = ctx->lcells;   // CSR of this rank's strip, cell order (x - x0)*dimy + y
@@ -1805,6 +1856,12 @@ static int fetch_image(sm_context* ctx, std::vector<Sec32>& top, std::vector<Sec
 }
 
 int sm_section_count(sm_context* ctx, int64_t* n) {
+  if (ctx->group) {
+    int64_t total = 0, part = 0;
+    const int rc = grp_settled_each(ctx, [&](sm_context* c, int) { const int rc_ = sm_section_count(c, &part); total += part; return rc_; });
+    *n = total;
+    return rc;
+  }
   std::vector<Sec32> top, pool;
   int rc = fetch_image(ctx, top, pool);
   if (rc != SM_OK) return rc;
@@ -1820,6 +1877,7 @@ int sm_section_count(sm_context* ctx, int64_t* n) {
 
 int sm_download_columns(sm_context* ctx, int64_t capacity, int64_t* offsets, int32_t* type, double* size,
                         double* floor_, double* saturation) {
+  if (ctx->group) return grp_download_columns(ctx, capacity, offsets, type, size, floor_, saturation);
   std::vector<Sec32> top, pool;
   int rc = fetch_image(ctx, top, pool);
   if (rc != SM_OK) return rc;
@@ -1850,6 +1908,7 @@ int sm_download_columns(sm_context* ctx, int64_t capacity, int64_t* offsets, int
 }
 
 int sm_download_height(sm_context* ctx, double* height) {
+  if (ctx->group) return grp_settled_each(ctx, [&](sm_context* c, int) { return sm_download_height(c, height + (size_t)c->x0 * c->d.dimy); });
   CK(cudaSetDevice(ctx->cfg.device));
   k_heights<<<ctx->num_sms * 8, 256, 0, ctx->stream>>>(ctx->d.top, ctx->d_scratch, nullptr, ctx->lcells);
   ctx->launches++;
@@ -1860,6 +1919,7 @@ int sm_download_height(sm_context* ctx, double* height) {
 }
 
 int sm_download_surface(sm_context* ctx, int32_t* surface) {
+  if (ctx->group) return grp_settled_each(ctx, [&](sm_context* c, int) { return sm_download_surface(c, surface + (size_t)c->x0 * c->d.dimy); });
   CK(cudaSetDevice(ctx->cfg.device));
   k_heights<<<ctx->num_sms * 8, 256, 0, ctx->stream>>>(ctx->d.top, nullptr, ctx->d_iscratch, ctx->lcells);
   ctx->launches++;
@@ -1869,9 +1929,11 @@ int sm_download_surface(sm_context* ctx, int32_t* surface) {
   return SM_OK;
 }
 
-int sm_height_sum(sm_context* ctx, double* sum) {
+// whole_map: a rank of a sharded map sums every strip through the peer pointers (the caller has settled the ranks)
+static int height_sum(sm_context* ctx, bool whole_map, double* sum) {
   CK(cudaSetDevice(ctx->cfg.device));
-  k_height_sum1<<<SUM_BLOCKS, 256, 0, ctx->stream>>>(ctx->d.top, ctx->lcells, ctx->d_scratch);
+  if (whole_map) k_height_sum1<true><<<SUM_BLOCKS, 256, 0, ctx->stream>>>(ctx->d, ctx->cells, ctx->d_scratch);
+  else k_height_sum1<false><<<SUM_BLOCKS, 256, 0, ctx->stream>>>(ctx->d, ctx->lcells, ctx->d_scratch);
   k_height_sum2<<<1, 256, 0, ctx->stream>>>(ctx->d_scratch, ctx->d_scratch + SUM_BLOCKS);
   ctx->launches += 2;
   CK(cudaGetLastError());
@@ -1879,8 +1941,19 @@ int sm_height_sum(sm_context* ctx, double* sum) {
   CK(cudaStreamSynchronize(ctx->stream));
   return SM_OK;
 }
+int sm_height_sum(sm_context* ctx, double* sum) {
+  if (ctx->group) return grp_settled_rank0(ctx, [&](sm_context* c) { return height_sum(c, true, sum); });
+  return height_sum(ctx, false, sum);
+}
 
 int sm_checksum(sm_context* ctx, uint64_t* out) {
+  if (ctx->group) {     // the strips' checksums add up mod 2^64
+    if (!out) return fail(ctx, SM_ERR_INVALID, "null argument");
+    uint64_t total = 0, part = 0;
+    const int rc = grp_settled_each(ctx, [&](sm_context* c, int) { const int rc_ = sm_checksum(c, &part); total += part; return rc_; });
+    *out = total;
+    return rc;
+  }
   if (!out) return fail(ctx, SM_ERR_INVALID, "null argument");
   CK(cudaSetDevice(ctx->cfg.device));
   unsigned long long* d_out = (unsigned long long*)(ctx->d_scratch + SUM_BLOCKS + 1);
@@ -1894,6 +1967,7 @@ int sm_checksum(sm_context* ctx, uint64_t* out) {
 }
 
 int sm_get_frequency(sm_context* ctx, float* wf, float* wt, float* windf) {
+  if (ctx->group) { float* const h[3] = {wf, wt, windf}; return grp_frequency(ctx, false, h); }
   CK(cudaSetDevice(ctx->cfg.device));
   CK(cudaStreamSynchronize(ctx->stream));
   if (wf) CK(cudaMemcpy(wf, ctx->d.wfreq, ctx->cells * 4, cudaMemcpyDeviceToHost));
@@ -1902,6 +1976,7 @@ int sm_get_frequency(sm_context* ctx, float* wf, float* wt, float* windf) {
   return SM_OK;
 }
 int sm_set_frequency(sm_context* ctx, const float* wf, const float* wt, const float* windf) {
+  if (ctx->group) { float* const h[3] = {(float*)wf, (float*)wt, (float*)windf}; return grp_frequency(ctx, true, h); }
   CK(cudaSetDevice(ctx->cfg.device));
   CK(cudaStreamSynchronize(ctx->stream));
   if (wf) CK(cudaMemcpy(ctx->d.wfreq, wf, ctx->cells * 4, cudaMemcpyHostToDevice));
@@ -1910,6 +1985,7 @@ int sm_set_frequency(sm_context* ctx, const float* wf, const float* wt, const fl
   return SM_OK;
 }
 int sm_frequency_update(sm_context* ctx) {
+  if (ctx->group) return grp_each(ctx, [&](sm_context* c, int) { return sm_frequency_update(c); });
   CK(cudaSetDevice(ctx->cfg.device));
   k_frequency_update<<<ctx->num_sms * 8, 256, 0, ctx->stream>>>(ctx->d.wfreq, ctx->d.wtrack, ctx->cells);
   ctx->launches++;
@@ -1924,6 +2000,7 @@ static int peers_ready(sm_context* ctx) {
   return SM_OK;
 }
 static int cell_op(sm_context* ctx, const CellOp& o, CellRes* out) {
+  if (ctx->group) return grp_cell_op(ctx, o, out);
   if (ctx->nsoils < 1) return fail(ctx, SM_ERR_INVALID, "soil table not set");
   const bool read = o.op == 3 || o.op == 4;
   if (ctx->nranks > 1 && !read) return fail(ctx, SM_ERR_INVALID, "single-cell operations are not available on a sharded context");
@@ -1981,6 +2058,7 @@ int sm_cell_water_cascade(sm_context* ctx, int32_t x, int32_t y, int32_t spill) 
 }
 int sm_cell_column(sm_context* ctx, int32_t x, int32_t y, int32_t capacity, int32_t* n, int32_t* type, double* size,
                    double* floor_, double* saturation) {
+  if (ctx->group) return grp_settled_rank0(ctx, [&](sm_context* c) { return sm_cell_column(c, x, y, capacity, n, type, size, floor_, saturation); });
   if (!inb(ctx, x, y) || !n || capacity < 0) return fail(ctx, SM_ERR_INVALID, "sm_cell_column: range");
   int rc = peers_ready(ctx);
   if (rc != SM_OK) return rc;
@@ -2011,6 +2089,7 @@ int sm_cell_column(sm_context* ctx, int32_t x, int32_t y, int32_t capacity, int3
   return SM_OK;
 }
 int sm_set_volume_factor(sm_context* ctx, double v) {
+  if (ctx->group) return grp_each(ctx, [&](sm_context* c, int) { return sm_set_volume_factor(c, v); });
   if (!(v > 0.0)) return fail(ctx, SM_ERR_INVALID, "sm_set_volume_factor: must be positive");
   ctx->d.volume_factor = v;
   return SM_OK;
@@ -2188,6 +2267,7 @@ static int zero_counters(sm_context* ctx) {
 }
 
 int sm_last_stats(sm_context* ctx, sm_stats* st) {
+  if (ctx->group) return grp_last_stats(ctx, st);
   CK(cudaSetDevice(ctx->cfg.device));
   // only the counters travel: barrier .. bump (SM_STATS_READBACK_BYTES, what bench.py counts as d2h per batch)
   static_assert(offsetof(RunCtl, ring) == 88, "bench.py counts 88 bytes read back per batch");
@@ -2217,6 +2297,10 @@ static int new_batch(sm_context* ctx, int kind, int n) {
 }
 
 static int run_host(sm_context* ctx, int kind, int n, const float* spawn_xy, int max_sweeps, sm_stats* st) {
+  if (ctx->group) {
+    const int rc = grp_run(ctx, kind, n, spawn_xy, nullptr, max_sweeps, true);
+    return rc != SM_OK ? rc : grp_last_stats(ctx, st);
+  }
   if (n > 0 && !spawn_xy) return fail(ctx, SM_ERR_INVALID, "null spawn list");
   if (ctx->nranks > 1 && ctx->share > 1)
     return fail(ctx, SM_ERR_INVALID, "contexts sharing a device must use sm_*_run_device on every rank, then sm_last_stats");
@@ -2234,6 +2318,7 @@ static int run_host(sm_context* ctx, int kind, int n, const float* spawn_xy, int
 
 // ---- mass budget (SURVEY.md A.7) --------------------------------------------------------------------------
 int sm_budget_particles(sm_context* ctx, int32_t n, double* out) {
+  if (ctx->group) return grp_budget_particles(ctx, n, out);
   if (!ctx->d.bud) return fail(ctx, SM_ERR_INVALID, "context was created without SM_FLAG_BUDGET");
   if (n < 0 || n > ctx->max_particles || (n && !out)) return fail(ctx, SM_ERR_INVALID, "sm_budget_particles: range");
   CK(cudaSetDevice(ctx->cfg.device));
@@ -2256,6 +2341,12 @@ int sm_last_budget(sm_context* ctx, sm_budget* out) {
 }
 
 int sm_last_cell_budget(sm_context* ctx, double* eroded, double* deposited, double* cascade_net) {
+  if (ctx->group)
+    return grp_settled_each(ctx, [&](sm_context* c, int) {
+      const size_t lo = (size_t)c->x0 * c->d.dimy;
+      return sm_last_cell_budget(c, eroded ? eroded + lo : nullptr, deposited ? deposited + lo : nullptr,
+                                 cascade_net ? cascade_net + lo : nullptr);
+    });
   if (!ctx->d_cells) return fail(ctx, SM_ERR_INVALID, "context was created without SM_FLAG_CELL_BUDGET");
   if (ctx->cells_state == 0) return fail(ctx, SM_ERR_INVALID, "no batch yet");
   if (ctx->cells_state == 2)
@@ -2277,6 +2368,7 @@ int sm_wind_run(sm_context* ctx, int32_t n, const float* xy, int32_t max_sweeps,
   return run_host(ctx, KIND_WIND, n, xy, max_sweeps, st);
 }
 int sm_water_run_device(sm_context* ctx, int32_t n, const float* d_xy, int32_t max_sweeps) {
+  if (ctx->group) return grp_run(ctx, KIND_WATER, n, nullptr, d_xy, max_sweeps, true);
   int rc = zero_counters(ctx);
   if (rc != SM_OK) return rc;
   rc = new_batch(ctx, KIND_WATER, n);
@@ -2284,6 +2376,7 @@ int sm_water_run_device(sm_context* ctx, int32_t n, const float* d_xy, int32_t m
   return launch_run(ctx, KIND_WATER, n, d_xy, max_sweeps);
 }
 int sm_wind_run_device(sm_context* ctx, int32_t n, const float* d_xy, int32_t max_sweeps) {
+  if (ctx->group) return grp_run(ctx, KIND_WIND, n, nullptr, d_xy, max_sweeps, true);
   int rc = zero_counters(ctx);
   if (rc != SM_OK) return rc;
   rc = new_batch(ctx, KIND_WIND, n);
@@ -2356,10 +2449,15 @@ static int hydro_cells_reset(sm_context* ctx) {
   return SM_OK;
 }
 int sm_hydro_issuer(sm_context* ctx, int32_t on) {
+  if (ctx->group) return fail(ctx, SM_ERR_INVALID, "a group issues the pooling hydrology from its rank 0");
   ctx->hydro_issuer = on != 0;
   return SM_OK;
 }
 int sm_water_flood(sm_context* ctx, sm_hydro_stats* st) {
+  if (ctx->group) {
+    if (ctx->cur_kind != KIND_WATER) return fail(ctx, SM_ERR_INVALID, "sm_water_flood: the last batch was not a water batch");
+    return grp_hydro(ctx, [&](sm_context* c) { return sm_water_flood(c, st); });
+  }
   int rc = hydro_ready(ctx);
   if (rc != SM_OK) return rc;
   if (ctx->cur_kind != KIND_WATER) return fail(ctx, SM_ERR_INVALID, "sm_water_flood: the last batch was not a water batch");
@@ -2380,6 +2478,7 @@ int sm_water_flood(sm_context* ctx, sm_hydro_stats* st) {
   return hydro_finish(ctx, st);
 }
 int sm_seep(sm_context* ctx, sm_hydro_stats* st) {
+  if (ctx->group) return grp_hydro(ctx, [&](sm_context* c) { return sm_seep(c, st); });
   int rc = hydro_ready(ctx);
   if (rc != SM_OK) return rc;
   ActiveMap am{};
@@ -2421,6 +2520,7 @@ int sm_seep(sm_context* ctx, sm_hydro_stats* st) {
   return rc2;
 }
 int sm_last_hydro_budget(sm_context* ctx, sm_hydro_budget* out) {
+  if (ctx->group) return grp_rank0(ctx, [&](sm_context* c) { return sm_last_hydro_budget(c, out); });
   if (!out) return fail(ctx, SM_ERR_INVALID, "null argument");
   if (!ctx->d.bud) return fail(ctx, SM_ERR_INVALID, "context was created without SM_FLAG_BUDGET");
   if (!ctx->hydro_bud_valid) return fail(ctx, SM_ERR_INVALID, "no hydrology call yet");
@@ -2459,6 +2559,7 @@ int sm_wind_begin(sm_context* ctx, int32_t n, const float* xy) {
   return run_host(ctx, KIND_WIND, n, xy, SM_SWEEPS_NONE, nullptr);
 }
 static int sweeps_k(sm_context* ctx, int kind, int k, sm_stats* st) {
+  if (ctx->group) return grp_sweeps(ctx, kind, k, st);
   if (ctx->cur_kind != kind) return fail(ctx, SM_ERR_INVALID, "no batch of this kind in flight");
   if (k <= 0) return fail(ctx, SM_ERR_INVALID, "k must be positive");
   int rc = zero_counters(ctx);
@@ -2473,6 +2574,7 @@ int sm_wind_sweeps(sm_context* ctx, int32_t k, sm_stats* st) { return sweeps_k(c
 static int fetch_state(sm_context* ctx, int kind, std::vector<float4>& a, std::vector<double2>& b,
                        std::vector<uint2>& c, std::vector<unsigned char>& al) {
   if (ctx->cur_kind != kind) return fail(ctx, SM_ERR_INVALID, "no batch of this kind in flight");
+  if (ctx->group) return grp_fetch_state(ctx, a, b, c, al);
   CK(cudaSetDevice(ctx->cfg.device));
   CK(cudaStreamSynchronize(ctx->stream));
   const size_t n = (size_t)ctx->cur_n;
@@ -2519,6 +2621,7 @@ int sm_wind_state(sm_context* ctx, float* pos2, float* speed3, double* height, d
 }
 
 int sm_set_soil_colors(sm_context* ctx, const float* rgba, int32_t n) {
+  if (ctx->group) return grp_each(ctx, [&](sm_context* c, int) { return sm_set_soil_colors(c, rgba, n); });
   if (!rgba || n < 1 || n > SM_MAX_SOILS) return fail(ctx, SM_ERR_INVALID, "sm_set_soil_colors: 1..64 soils");
   CK(cudaSetDevice(ctx->cfg.device));
   if (!ctx->d_colors) CK(cudaMalloc(&ctx->d_colors, SM_MAX_SOILS * sizeof(float4)));
@@ -2526,6 +2629,10 @@ int sm_set_soil_colors(sm_context* ctx, const float* rgba, int32_t n) {
   return SM_OK;
 }
 int sm_mesh_update(sm_context* ctx, int32_t slice, float* host_vertices) {
+  if (ctx->group)
+    return grp_settled_each(ctx, [&](sm_context* c, int) {
+      return sm_mesh_update(c, slice, host_vertices ? host_vertices + (size_t)c->x0 * c->d.dimy * 11 : nullptr);
+    });
   if (!ctx->d_colors) return fail(ctx, SM_ERR_INVALID, "sm_mesh_update: soil colours not set");
   int rc = peers_ready(ctx);
   if (rc != SM_OK) return rc;
@@ -2546,6 +2653,9 @@ int sm_mesh_update(sm_context* ctx, int32_t slice, float* host_vertices) {
   return SM_OK;
 }
 int sm_mesh_device_ptr(sm_context* ctx, void** dptr) {
+  if (ctx->group)
+    return fail(ctx, SM_ERR_INVALID, "sm_mesh_device_ptr: a group of several ranks has no single device array "
+                                     "(sm_group_rank gives the ranks, each with its strip's pointer)");
   if (!ctx->mesh_valid) return fail(ctx, SM_ERR_INVALID, "no mesh yet: call sm_mesh_update");
   *dptr = ctx->d_verts;
   return SM_OK;
@@ -2567,10 +2677,12 @@ static int export_maps(sm_context* ctx, float* height, float* bgra) {
 }
 int sm_export_height(sm_context* ctx, float* height) {
   if (!height) return fail(ctx, SM_ERR_INVALID, "null buffer");
+  if (ctx->group) return grp_each(ctx, [&](sm_context* c, int) { return sm_export_height(c, height + (size_t)c->x0 * c->d.dimy); });
   return export_maps(ctx, height, nullptr);
 }
 int sm_export_color(sm_context* ctx, float* bgra) {
   if (!bgra) return fail(ctx, SM_ERR_INVALID, "null buffer");
+  if (ctx->group) return grp_each(ctx, [&](sm_context* c, int) { return sm_export_color(c, bgra + (size_t)c->x0 * c->d.dimy * 4); });
   return export_maps(ctx, nullptr, bgra);
 }
 int sm_parse_soil_file(const char* path, sm_soil* soils, char* names, float* colors, int32_t max_soils,
@@ -2610,6 +2722,7 @@ static int lbm_ready(sm_context* ctx) {
   return SM_OK;
 }
 int sm_lbm_init(sm_context* ctx) {
+  if (ctx->group) return grp_each(ctx, [&](sm_context* c, int) { return sm_lbm_init(c); });
   int rc = lbm_ready(ctx);
   if (rc != SM_OK) return rc;
   ctx->lbm_cur = 0;
@@ -2619,6 +2732,7 @@ int sm_lbm_init(sm_context* ctx) {
   return SM_OK;
 }
 int sm_lbm_create(sm_context* ctx, int32_t nx, int32_t ny, int32_t nz) {
+  if (ctx->group) return grp_each(ctx, [&](sm_context* c, int) { return sm_lbm_create(c, nx, ny, nz); });
   if (nx < 3 || ny < 3 || nz < 3 || (int64_t)nx * ny * nz * LBM_Q >= (1ll << 31))
     return fail(ctx, SM_ERR_INVALID, "sm_lbm_create: 3 <= nx, ny, nz and nx*ny*nz*19 < 2^31");
   CK(cudaSetDevice(ctx->cfg.device));
@@ -2647,6 +2761,10 @@ int sm_lbm_create(sm_context* ctx, int32_t nx, int32_t ny, int32_t nz) {
   return sm_lbm_init(ctx);       // lbmwind.h:101-107: init.cs runs while the boundary is still all zero
 }
 int sm_lbm_set_boundary(sm_context* ctx, const float* boundary) {
+  if (ctx->group) {     // from the terrain: every rank reads the whole map
+    const int rc = boundary ? SM_OK : grp_settle(ctx);
+    return rc != SM_OK ? rc : grp_each(ctx, [&](sm_context* c, int) { return sm_lbm_set_boundary(c, boundary); });
+  }
   int rc = lbm_ready(ctx);
   if (rc != SM_OK) return rc;
   const size_t n = (size_t)ctx->lbm.nx * ctx->lbm.ny * ctx->lbm.nz;
@@ -2664,6 +2782,12 @@ int sm_lbm_set_boundary(sm_context* ctx, const float* boundary) {
   return SM_OK;
 }
 int sm_lbm_step(sm_context* ctx, int32_t nsteps, double* device_ms) {
+  if (ctx->group) {     // every rank steps its copy of the lattice; the slowest rank's time
+    double worst = 0.0, ms = 0.0;
+    const int rc = grp_each(ctx, [&](sm_context* c, int) { const int rc_ = sm_lbm_step(c, nsteps, &ms); worst = std::max(worst, ms); return rc_; });
+    if (device_ms) *device_ms = worst;
+    return rc;
+  }
   int rc = lbm_ready(ctx);
   if (rc != SM_OK) return rc;
   if (nsteps < 0) return fail(ctx, SM_ERR_INVALID, "sm_lbm_step: nsteps");
@@ -2684,6 +2808,7 @@ int sm_lbm_step(sm_context* ctx, int32_t nsteps, double* device_ms) {
   return SM_OK;
 }
 int sm_lbm_get(sm_context* ctx, float* f, float* rho, float* v4) {
+  if (ctx->group) return grp_rank0(ctx, [&](sm_context* c) { return sm_lbm_get(c, f, rho, v4); });
   int rc = lbm_ready(ctx);
   if (rc != SM_OK) return rc;
   CK(cudaStreamSynchronize(ctx->stream));
@@ -2698,6 +2823,7 @@ int sm_lbm_get(sm_context* ctx, float* f, float* rho, float* v4) {
   return SM_OK;
 }
 int sm_wind_use_lbm(sm_context* ctx, int32_t on) {
+  if (ctx->group) return grp_each(ctx, [&](sm_context* c, int) { return sm_wind_use_lbm(c, on); });
   if (!on) { ctx->d.wind_v4 = nullptr; return SM_OK; }
   int rc = lbm_ready(ctx);
   if (rc != SM_OK) return rc;
@@ -2706,6 +2832,7 @@ int sm_wind_use_lbm(sm_context* ctx, int32_t on) {
   return SM_OK;
 }
 int sm_lbm_advect(sm_context* ctx, int32_t n, float* pos4) {
+  if (ctx->group) return grp_rank0(ctx, [&](sm_context* c) { return sm_lbm_advect(c, n, pos4); });
   int rc = lbm_ready(ctx);
   if (rc != SM_OK) return rc;
   if (n < 0 || (n && !pos4)) return fail(ctx, SM_ERR_INVALID, "sm_lbm_advect: arguments");
@@ -2725,11 +2852,13 @@ int sm_lbm_advect(sm_context* ctx, int32_t n, float* pos4) {
 }
 
 int sm_timer_start(sm_context* ctx) {
+  if (ctx->group) return grp_rank0(ctx, [&](sm_context* c) { return sm_timer_start(c); });
   CK(cudaSetDevice(ctx->cfg.device));
   CK(cudaEventRecord(ctx->evt0, ctx->stream));
   return SM_OK;
 }
 int sm_timer_stop(sm_context* ctx, double* elapsed_ms) {
+  if (ctx->group) return grp_rank0(ctx, [&](sm_context* c) { return sm_timer_stop(c, elapsed_ms); });
   CK(cudaSetDevice(ctx->cfg.device));
   CK(cudaEventRecord(ctx->evt1, ctx->stream));
   CK(cudaEventSynchronize(ctx->evt1));
@@ -2738,11 +2867,16 @@ int sm_timer_stop(sm_context* ctx, double* elapsed_ms) {
   if (elapsed_ms) *elapsed_ms = ms;
   return SM_OK;
 }
-int sm_launch_count(sm_context* ctx, int64_t* n) { *n = ctx->launches; return SM_OK; }
+int sm_launch_count(sm_context* ctx, int64_t* n) {
+  *n = ctx->launches;
+  if (ctx->group) for (int r = 0; r < ctx->group->n; r++) *n += ctx->group->rank[r]->launches;
+  return SM_OK;
+}
 // debug (only meaningful in a -DSM_PROFILE build): clock64() totals per phase, summed over particles
 // -DSM_PROFILE builds of k_sweep: 8 words per sweep - live particles, max step cycles, max wait cycles, max cycles a
 // warp spent on its particles, sum of step cycles, steps, globaltimer at the first warp's start, at the last warp's end
 int sm_debug_sweeps8(sm_context* ctx, uint64_t* out, int nsweeps) {
+  if (ctx->group) return grp_rank0(ctx, [&](sm_context* c) { return sm_debug_sweeps8(c, out, nsweeps); });
   CK(cudaSetDevice(ctx->cfg.device));
   CK(cudaStreamSynchronize(ctx->stream));
   CK(cudaMemcpy(out, ctx->d.dbg, (size_t)std::min(nsweeps, 16384) * 64, cudaMemcpyDeviceToHost));
@@ -2750,12 +2884,14 @@ int sm_debug_sweeps8(sm_context* ctx, uint64_t* out, int nsweeps) {
   return SM_OK;
 }
 int sm_debug_sweeps(sm_context* ctx, uint64_t* out, int nsweeps) {   // -DSM_PROFILE builds: (clock64, alive) per sweep
+  if (ctx->group) return grp_rank0(ctx, [&](sm_context* c) { return sm_debug_sweeps(c, out, nsweeps); });
   CK(cudaSetDevice(ctx->cfg.device));
   CK(cudaStreamSynchronize(ctx->stream));
   CK(cudaMemcpy(out, ctx->d.dbg, (size_t)std::min(nsweeps, 16384) * 16, cudaMemcpyDeviceToHost));
   return SM_OK;
 }
 int sm_debug_profile(sm_context* ctx, uint64_t* out16, int reset) {
+  if (ctx->group) return grp_rank0(ctx, [&](sm_context* c) { return sm_debug_profile(c, out16, reset); });
   CK(cudaSetDevice(ctx->cfg.device));
   CK(cudaStreamSynchronize(ctx->stream));
   RunCtl h;
@@ -2769,16 +2905,19 @@ int sm_debug_profile(sm_context* ctx, uint64_t* out16, int reset) {
   return SM_OK;
 }
 int sm_device_alloc(sm_context* ctx, int64_t bytes, void** dptr) {
+  if (ctx->group) return grp_rank0(ctx, [&](sm_context* c) { return sm_device_alloc(c, bytes, dptr); });
   CK(cudaSetDevice(ctx->cfg.device));
   CK(cudaMalloc(dptr, (size_t)bytes));
   return SM_OK;
 }
 int sm_device_free(sm_context* ctx, void* dptr) {
+  if (ctx->group) return grp_rank0(ctx, [&](sm_context* c) { return sm_device_free(c, dptr); });
   CK(cudaSetDevice(ctx->cfg.device));
   CK(cudaFree(dptr));
   return SM_OK;
 }
 int sm_device_upload(sm_context* ctx, void* dptr, const void* host, int64_t bytes) {
+  if (ctx->group) return grp_rank0(ctx, [&](sm_context* c) { return sm_device_upload(c, dptr, host, bytes); });
   CK(cudaSetDevice(ctx->cfg.device));
   CK(cudaMemcpyAsync(dptr, host, (size_t)bytes, cudaMemcpyHostToDevice, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
@@ -2786,6 +2925,7 @@ int sm_device_upload(sm_context* ctx, void* dptr, const void* host, int64_t byte
 }
 
 int sm_initialize(sm_context* ctx, int32_t seed, const sm_layer* layers, int32_t nlayers) {
+  if (ctx->group) return grp_each(ctx, [&](sm_context* c, int) { return sm_initialize(c, seed, layers, nlayers); });
   if (!layers || nlayers < 1 || nlayers > SM_MAX_LAYERS)
     return fail(ctx, SM_ERR_INVALID, "sm_initialize: 1..16 layers");
   CK(cudaSetDevice(ctx->cfg.device));

@@ -44,7 +44,10 @@ def spawn_list(n, dimx, dimy):
 class Simulation:
     """soil preset + GPU context + frame loop."""
 
-    def __init__(self, soil, seed=42, dimx=0, dimy=0, device=0, max_particles=0, pool_capacity=0):
+    def __init__(self, soil, seed=42, dimx=0, dimy=0, device=0, max_particles=0, pool_capacity=0, gpus=1,
+                 devices=None, budget=False, cell_budget=False):
+        """gpus / devices: the map sharded over several GPUs of this process (capi.Context); the frame loop is the
+        same.  budget / cell_budget: keep the mass budgets (capi.Context)."""
         # a preset name (JSON tables dumped from the reference loader) or a path to a `.soil` file
         self.preset = capi.parse_soil_file(soil) if str(soil).endswith(".soil") and os.path.exists(str(soil)) \
             else presets.load(soil)
@@ -55,7 +58,8 @@ class Simulation:
         self.seed = int(seed)
         srand(self.seed)                                   # SoilMachine.cpp:41
         self.ctx = capi.Context(self.dimx, self.dimy, self.scale, device=device,
-                                pool_capacity=pool_capacity, max_particles=max_particles)
+                                pool_capacity=pool_capacity, max_particles=max_particles, gpus=gpus, devices=devices,
+                                budget=budget, cell_budget=cell_budget)
         self.ctx.set_soils(self.preset["soils"])
         self.ctx.set_soil_colors(self.preset["colors"])
         self.ctx.initialize(self.seed, self.preset["layers"])   # Layermap(SEED, dim), SoilMachine.cpp:83
