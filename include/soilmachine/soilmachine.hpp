@@ -235,6 +235,33 @@ class Layermap {
   template <class VP> void slice(VP& vp, double s) { slice_plane = (int)s; update(vp); }                     // :557-
   template <class VP> void slice(VP& vp) { update(vp); }
 
+  // ---- snapshots (what io.h:232 asks for: "Should be able to also WRITE to file!!") -------------------------------
+  // save() writes the snapshot of the whole map - columns and frequency arrays, format in soilmachine_b200.h - to a
+  // file; load() restores it, on one GPU or several, whichever wrote it.  The soil table must be the one of the saving
+  // run (loadsoil of the same file).  The application keeps its own rand() stream, as upstream does.
+  void save(const std::string& path) {
+    int64_t n = 0;
+    ck(sm_snapshot_bytes(ctx, &n));
+    std::vector<unsigned char> buf((size_t)n);
+    ck(sm_snapshot_save(ctx, buf.data(), n, 0));
+    std::FILE* f = std::fopen(path.c_str(), "wb");
+    if (!f) throw Error(SM_ERR_INVALID, "Layermap::save: cannot open " + path);
+    const size_t w = std::fwrite(buf.data(), 1, buf.size(), f);
+    if (std::fclose(f) != 0 || w != buf.size()) throw Error(SM_ERR_INVALID, "Layermap::save: cannot write " + path);
+  }
+  void load(const std::string& path) {
+    std::FILE* f = std::fopen(path.c_str(), "rb");
+    if (!f) throw Error(SM_ERR_INVALID, "Layermap::load: cannot open " + path);
+    std::vector<unsigned char> buf;
+    unsigned char chunk[1 << 16];
+    for (size_t r; (r = std::fread(chunk, 1, sizeof(chunk), f)) > 0;) buf.insert(buf.end(), chunk, chunk + r);
+    std::fclose(f);
+    push_tables();
+    touch();
+    const int rc = sm_snapshot_restore(ctx, buf.data(), (int64_t)buf.size(), 0);
+    if (rc != SM_OK) throw Error(rc, sm_last_error(ctx));
+  }
+
   // every call that may change columns goes through here
   void touch() { mirror_valid = false; mirror_reads = 0; mesh_stale = true; }
 

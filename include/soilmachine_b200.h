@@ -196,6 +196,49 @@ int sm_height_sum(sm_context* ctx, double* sum);             /* deterministic tr
  * whole map.  soilmachine_b200/checksum.py computes the same number from downloaded / reference columns. */
 int sm_checksum(sm_context* ctx, uint64_t* checksum);
 
+/* ---- snapshots: one canonical byte image of the columns and the frequency arrays ------------------------------------
+ * The reference can only read a map from files (io.h:232: "Should be able to also WRITE to file!!").  A snapshot
+ * (format version 1, little-endian, DESIGN.md section 10) covers the x-range [x0, x1) of the map:
+ *   header, 128 B: magic "SMSNAP\0\0"; u32 version = 1, header_bytes = 128; i32 dimx, dimy, x0, x1, nsoils,
+ *                  reserved = 0; u64 ncells = (x1 - x0)*dimy, nsections, offsets_at, records_at, freq_at, total_bytes,
+ *                  checksum (sm_checksum of the covered columns, global cell indices); zeros up to 128 B
+ *   offsets:       u64[ncells + 1] at offsets_at = 128, cell order (x - x0)*dimy + y: the CSR of sm_download_columns
+ *   records:       at records_at (32-B aligned): nsections x {f64 size, floor, saturation; u32 type, reserved = 0},
+ *                  bottom -> top within each column; floor is stored as it is, not recomputed on restore
+ *   frequency:     f32 water_frequency, water_track, wind_frequency, each [dimy][x1 - x0]
+ * It is canonical: contexts whose columns and frequency arrays are equal byte for byte write identical snapshots,
+ * whatever their pool history and sharding.  NOT in a snapshot: the soil table and colours (the application sets
+ * them; nsoils must match), the volume factor, the lattice and sm_wind_use_lbm, particle state and any open batch,
+ * budgets and per-cell maps.
+ * Who saves and restores what:
+ *   a plain context: whole-map snapshots;
+ *   a rank of a sharded map (sm_create_sharded): saves the snapshot of its own strip; restores a whole-map snapshot
+ *     (its own slice of columns and frequency columns) or a strip snapshot of exactly its range.  Every rank's
+ *     earlier work must have completed before any rank restores, every rank restores before the next batch, and each
+ *     rank writes only its own strip.  The strips of a cut concatenate into the whole-map snapshot
+ *     (soilmachine_b200/snapshot.py: join / cut);
+ *   a group (sm_create_group): whole-map snapshots, every rank saving or restoring its slice.
+ * So a snapshot taken on one GPU restores on any number of them, and the reverse.
+ * sm_snapshot_bytes: the size sm_snapshot_save would write now (runs the count pass on the device).
+ * sm_snapshot_save: dst is host memory (pageable or pinned) or, dst_on_device != 0, device memory on the context's
+ *   device (rank 0's for a group), e.g. from sm_device_alloc.  SM_ERR_INVALID when capacity is too small.  A save to
+ *   host memory needs the offsets array and a 32 MB staging buffer of extra device memory, never a copy of the map.
+ * sm_snapshot_restore: the context's columns and frequency arrays (over the snapshot's range) become the snapshot's.
+ *   Everything is validated before anything is written - the header (magic, version, dimensions, nsoils against the
+ *   soil table, which must be set, the x-range, bytes), the offsets (from 0, monotone, ending at nsections) and every
+ *   record (type < nsoils) - so a refused restore leaves the context as it was.  SM_ERR_POOL when a fixed
+ *   pool_capacity (or a sharded rank's pool) is too small; pool_capacity == 0 on one context grows the pool as
+ *   sm_upload_columns does.  A host source is copied to the device whole (offsets and records of the restored
+ *   range) before it is validated.  Afterwards the pool is compact (bump = buried sections, free rings empty), the
+ *   mesh is stale and no batch is open: sm_*_sweeps and sm_water_flood are refused until the next batch.
+ *   Last, the restored columns' checksum is compared with the header's where the context holds all the snapshot
+ *   covers (a plain context, a group, a rank restoring a strip snapshot of its range): SM_ERR_INVALID when they
+ *   differ, and the map then HOLDS WHAT THE DAMAGED SNAPSHOT DESCRIBES.  A rank restoring its slice of a whole-map
+ *   snapshot cannot check alone; the sum of the ranks' checksums must equal the header's (sharded.py does this). */
+int sm_snapshot_bytes(sm_context* ctx, int64_t* bytes);
+int sm_snapshot_save(sm_context* ctx, void* dst, int64_t capacity, int32_t dst_on_device);
+int sm_snapshot_restore(sm_context* ctx, const void* src, int64_t bytes, int32_t src_on_device);
+
 /* WaterParticle::frequency/track, WindParticle::frequency (water.h:345-346, wind.h:48).
  * Any pointer may be NULL. */
 int sm_get_frequency(sm_context* ctx, float* water_frequency, float* water_track, float* wind_frequency);

@@ -39,6 +39,7 @@ SYMBOLS = [
     "sm_peer_export", "sm_peer_attach", "sm_hydro_issuer", "sm_parse_soil_file", "sm_water_flood", "sm_seep", "sm_last_budget", "sm_budget_particles", "sm_last_cell_budget", "sm_last_hydro_budget", "sm_last_hydro_cell_budget", "sm_lbm_create", "sm_lbm_set_boundary", "sm_lbm_init",
     "sm_lbm_step", "sm_lbm_get", "sm_lbm_advect", "sm_wind_use_lbm",
     "sm_create_group", "sm_group_size", "sm_group_rank", "sm_group_layout",
+    "sm_snapshot_bytes", "sm_snapshot_save", "sm_snapshot_restore",
 ]
 
 
@@ -303,6 +304,40 @@ class Context:
 
     def frequency_update(self):
         self._ck(self.lib.sm_frequency_update(self.h))
+
+    # ---- snapshots (soilmachine_b200/snapshot.py has the format) ----------------------------------------------------
+    def snapshot_bytes(self):
+        n = C.c_int64()
+        self._ck_strict(self.lib.sm_snapshot_bytes(self.h, C.byref(n)))
+        return n.value
+
+    def snapshot(self):
+        """the snapshot of this context's columns and frequency arrays (its strip on a rank of a sharded map, the
+        whole map otherwise) as a np.uint8 array"""
+        out = np.empty(self.snapshot_bytes(), np.uint8)
+        self._ck_strict(self.lib.sm_snapshot_save(self.h, out.ctypes.data_as(C.c_void_p), C.c_int64(out.size), 0))
+        return out
+
+    def snapshot_device(self):
+        """the snapshot in device memory from sm_device_alloc: (dptr, nbytes); free it with device_free(dptr)"""
+        n = self.snapshot_bytes()
+        d = C.c_void_p()
+        self._ck_strict(self.lib.sm_device_alloc(self.h, C.c_int64(n), C.byref(d)))
+        rc = self.lib.sm_snapshot_save(self.h, d, C.c_int64(n), 1)
+        if rc != SM_OK:
+            self.lib.sm_device_free(self.h, d)
+            self._ck_strict(rc)
+        return d, n
+
+    def restore(self, buf):
+        """restore a snapshot: host bytes / a np.uint8 array, or (dptr, nbytes) of snapshot_device()"""
+        if isinstance(buf, tuple):
+            d, n = buf
+            self._ck_strict(self.lib.sm_snapshot_restore(self.h, C.c_void_p(d.value if isinstance(d, C.c_void_p) else d),
+                                                         C.c_int64(n), 1))
+            return
+        a = np.frombuffer(memoryview(buf), np.uint8)
+        self._ck_strict(self.lib.sm_snapshot_restore(self.h, a.ctypes.data_as(C.c_void_p), C.c_int64(a.size), 0))
 
     def set_soil_colors(self, rgba):
         rgba = np.ascontiguousarray(rgba, np.float32).reshape(-1, 4)

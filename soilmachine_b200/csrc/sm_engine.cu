@@ -20,6 +20,8 @@
 #include "sm_noise.cuh"
 #include "sm_hydro.cuh"
 #include "sm_lbm.cuh"
+#include "sm_snap.cuh"
+#include <cub/device/device_scan.cuh>
 
 #define KIND_WATER 0
 #define KIND_WIND 1
@@ -855,6 +857,49 @@ __global__ void __launch_bounds__(256) k_checksum(DevCtx c, unsigned long long* 
     __syncthreads();
   }
   if (threadIdx.x == 0) atomicAdd(out, sh[0]);
+}
+
+// ---- snapshots (sm_snap.cuh): one thread per cell of this context's strip -------------------------------------------
+// save: off[c] = length of column c (its own pool), off[cells] = 0; CUB's in-place exclusive scan turns this into the
+// offsets
+__global__ void __launch_bounds__(256) k_snap_count(DevCtx c, size_t cells, unsigned long long* __restrict__ off) {
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < cells; i += (size_t)gridDim.x * blockDim.x)
+    off[i] = snap_count_cell(c.top[i], c.pool);
+  if (blockIdx.x == 0 && threadIdx.x == 0) off[cells] = 0;
+}
+// save: the records of cells [lo, hi), bottom -> top, at out[off[c] - off[lo]]
+__global__ void __launch_bounds__(256) k_snap_pack(DevCtx c, const unsigned long long* __restrict__ off, size_t lo,
+                                                   size_t hi, SnapRec* __restrict__ out) {
+  const unsigned long long base = off[lo];
+  for (size_t i = lo + (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < hi; i += (size_t)gridDim.x * blockDim.x)
+    snap_pack_cell(c.top[i], c.pool, off[i + 1] - off[i], out + (off[i] - base));
+}
+// save: out[i] = off[i] + add for i <= n (a rank's offsets placed in a whole-map snapshot)
+__global__ void __launch_bounds__(256) k_snap_offsets(const unsigned long long* __restrict__ off, size_t n,
+                                                      unsigned long long add, unsigned long long* __restrict__ out) {
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i <= n; i += (size_t)gridDim.x * blockDim.x)
+    out[i] = off[i] + add;
+}
+// restore, before any map write: reads the snapshot's slice only.  err[0] |= 1 on a bad cell; buried[c] = the pool slots
+// column c needs, buried[cells] = 0, for the in-place exclusive scan that gives each column its pool base
+__global__ void __launch_bounds__(256) k_snap_validate(const unsigned long long* __restrict__ off,
+                                                       const SnapRec* __restrict__ rec, size_t cells, int nsoils,
+                                                       unsigned long long* __restrict__ buried, unsigned int* err) {
+  bool bad = false;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < cells; i += (size_t)gridDim.x * blockDim.x) {
+    const bool ok = snap_valid_cell((const uint64_t*)off, rec, cells, i, nsoils);
+    buried[i] = ok ? snap_buried((const uint64_t*)off, i) : 0;
+    bad |= !ok;
+  }
+  if (bad) atomicOr(err, 1u);
+  if (blockIdx.x == 0 && threadIdx.x == 0) buried[cells] = 0;
+}
+// restore: every column of the strip from its records; base = the scanned buried counts
+__global__ void __launch_bounds__(256) k_snap_unpack(DevCtx c, const unsigned long long* __restrict__ off,
+                                                     const SnapRec* __restrict__ rec, size_t cells,
+                                                     const unsigned long long* __restrict__ base) {
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < cells; i += (size_t)gridDim.x * blockDim.x)
+    snap_unpack_cell((const uint64_t*)off, rec, i, (uint32_t)base[i], c.top[i], c.pool);
 }
 
 // Layermap::initialize, layermap.h:163-216: one thread per cell replays add() for every layer
@@ -2954,6 +2999,291 @@ int sm_initialize(sm_context* ctx, int32_t seed, const sm_layer* layers, int32_t
   ctx->launches++;
   CK(cudaGetLastError());
   CK(cudaStreamSynchronize(ctx->stream));
+  return SM_OK;
+}
+
+// ---- snapshots (sm_snap.cuh, DESIGN.md section 10) ---------------------------------------------------------------
+// A save to host memory packs the records through this much device memory at a time, cell range by cell range.
+#define SNAP_STAGE_BYTES (32ull << 20)
+
+namespace {
+struct DevTmp {      // device allocations of one snapshot call, freed when the call returns
+  int device = 0;
+  std::vector<void*> p;
+  DevTmp() = default;
+  DevTmp(const DevTmp&) = delete;
+  DevTmp& operator=(const DevTmp&) = delete;
+  ~DevTmp() {
+    if (p.empty()) return;
+    cudaSetDevice(device);
+    for (void* q : p) cudaFree(q);
+  }
+};
+}  // namespace
+
+static int snap_alloc(sm_context* ctx, DevTmp& t, size_t bytes, void** out) {
+  t.device = ctx->cfg.device;
+  CK(cudaMalloc(out, std::max<size_t>(bytes, 32)));
+  t.p.push_back(*out);
+  return SM_OK;
+}
+// in-place exclusive sum of d[0, n)
+static int snap_scan(sm_context* ctx, DevTmp& t, unsigned long long* d, size_t n) {
+  size_t tb = 0;
+  CK(cub::DeviceScan::ExclusiveSum(nullptr, tb, d, d, (int64_t)n, ctx->stream));
+  void* tmp = nullptr;
+  const int rc = snap_alloc(ctx, t, tb, &tmp);
+  if (rc != SM_OK) return rc;
+  CK(cub::DeviceScan::ExclusiveSum(tmp, tb, d, d, (int64_t)n, ctx->stream));
+  ctx->launches += 2;      // CUB's initialisation and scan kernels
+  return SM_OK;
+}
+// the count pass: *d_off = the offsets of this context's strip on the device, *nsec = its sections
+static int snap_count(sm_context* ctx, DevTmp& t, unsigned long long** d_off, uint64_t* nsec) {
+  CK(cudaSetDevice(ctx->cfg.device));
+  int rc = snap_alloc(ctx, t, (ctx->lcells + 1) * 8, (void**)d_off);
+  if (rc != SM_OK) return rc;
+  k_snap_count<<<ctx->num_sms * 8, 256, 0, ctx->stream>>>(ctx->d, ctx->lcells, *d_off);
+  ctx->launches++;
+  CK(cudaGetLastError());
+  rc = snap_scan(ctx, t, *d_off, ctx->lcells + 1);
+  if (rc != SM_OK) return rc;
+  unsigned long long n = 0;
+  CK(cudaMemcpyAsync(&n, *d_off + ctx->lcells, 8, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  *nsec = n;
+  return SM_OK;
+}
+// the header and the zero gap before the records
+static int snap_put_header(sm_context* ctx, const SnapHeader& H, unsigned char* dst, bool dev) {
+  const size_t gap0 = H.offsets_at + 8 * (H.ncells + 1), gap = H.records_at - gap0;
+  if (!dev) {
+    memcpy(dst, &H, sizeof(H));
+    memset(dst + gap0, 0, gap);
+    return SM_OK;
+  }
+  CK(cudaSetDevice(ctx->cfg.device));
+  CK(cudaMemcpyAsync(dst, &H, sizeof(H), cudaMemcpyHostToDevice, ctx->stream));
+  if (gap) CK(cudaMemsetAsync(dst + gap0, 0, gap, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  return SM_OK;
+}
+// This context's strip into the snapshot H at dst: its offsets (plus sb, the sections of the snapshot's cells before
+// the strip), its records and its frequency columns.  d_off from snap_count.
+static int snap_put_strip(sm_context* ctx, DevTmp& t, const SnapHeader& H, uint64_t sb, unsigned char* dst, bool dev,
+                          const unsigned long long* d_off) {
+  CK(cudaSetDevice(ctx->cfg.device));
+  const size_t L = ctx->lcells, dimy = (size_t)ctx->d.dimy;
+  unsigned long long* const o_dst = (unsigned long long*)(dst + H.offsets_at) + (size_t)(ctx->x0 - H.x0) * dimy;
+  SnapRec* const r_dst = (SnapRec*)(dst + H.records_at) + sb;
+  if (dev) {
+    k_snap_offsets<<<ctx->num_sms * 8, 256, 0, ctx->stream>>>(d_off, L, sb, o_dst);
+    k_snap_pack<<<ctx->num_sms * 8, 256, 0, ctx->stream>>>(ctx->d, d_off, 0, L, r_dst);
+    ctx->launches += 2;
+    CK(cudaGetLastError());
+  } else {
+    CK(cudaMemcpyAsync(o_dst, d_off, (L + 1) * 8, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    if (sb) for (size_t i = 0; i <= L; i++) o_dst[i] += sb;
+    SnapRec* stage = nullptr;
+    const int rc = snap_alloc(ctx, t, SNAP_STAGE_BYTES, (void**)&stage);
+    if (rc != SM_OK) return rc;
+    const unsigned long long cap = SNAP_STAGE_BYTES / sizeof(SnapRec);
+    for (size_t lo = 0; lo < L;) {     // the longest cell range whose records fit in the staging buffer
+      const size_t hi = (size_t)(std::upper_bound(o_dst + lo + 1, o_dst + L + 1, o_dst[lo] + cap) - o_dst) - 1;
+      if (hi == lo) return fail(ctx, SM_ERR_INVALID, "sm_snapshot_save: a column longer than the staging buffer");
+      k_snap_pack<<<ctx->num_sms * 8, 256, 0, ctx->stream>>>(ctx->d, d_off, lo, hi, stage);
+      ctx->launches++;
+      CK(cudaGetLastError());
+      const size_t n = (size_t)(o_dst[hi] - o_dst[lo]);
+      if (n) CK(cudaMemcpyAsync(r_dst + (o_dst[lo] - sb), stage, n * sizeof(SnapRec), cudaMemcpyDeviceToHost, ctx->stream));
+      CK(cudaStreamSynchronize(ctx->stream));
+      lo = hi;
+    }
+  }
+  const float* const src[3] = {ctx->d.wfreq, ctx->d.wtrack, ctx->d.windfreq};
+  const size_t w = (size_t)(H.x1 - H.x0);
+  for (int k = 0; k < 3; k++)
+    CK(cudaMemcpy2DAsync(dst + H.freq_at + (size_t)k * 4 * H.ncells + 4 * (size_t)(ctx->x0 - H.x0), 4 * w,
+                         src[k] + ctx->x0, 4 * (size_t)ctx->d.dimx, 4 * (size_t)(ctx->x1 - ctx->x0), dimy,
+                         cudaMemcpyDefault, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  return SM_OK;
+}
+
+// Save (dst != NULL) or size (bytes != NULL) the snapshot of this context: its strip, or the whole map of a group.
+static int snap_save(sm_context* ctx, int64_t* bytes, void* dst, int64_t capacity, bool dev) {
+  const int n = ctx->group ? ctx->group->n : 1;
+  sm_context* const* const R = ctx->group ? ctx->group->rank : &ctx;
+  if (ctx->group) {
+    const int rc = grp_settle(ctx);
+    if (rc != SM_OK) return rc;
+  } else {
+    CK(cudaSetDevice(ctx->cfg.device));
+    CK(cudaStreamSynchronize(ctx->stream));
+  }
+  std::vector<DevTmp> t((size_t)n);
+  std::vector<unsigned long long*> d_off((size_t)n, nullptr);
+  std::vector<uint64_t> base((size_t)n + 1, 0);
+  for (int r = 0; r < n; r++) {       // every rank counts; the rank totals become the section bases
+    uint64_t nsec = 0;
+    const int rc = snap_count(R[r], t[(size_t)r], &d_off[(size_t)r], &nsec);
+    if (rc != SM_OK) return ctx->group ? grp_err(ctx, r, rc) : rc;
+    base[(size_t)r + 1] = base[(size_t)r] + nsec;
+  }
+  SnapHeader H;
+  snap_layout(H, ctx->d.dimx, ctx->d.dimy, ctx->group ? 0 : ctx->x0, ctx->group ? ctx->d.dimx : ctx->x1, ctx->nsoils,
+              base[(size_t)n]);
+  if (bytes) { *bytes = (int64_t)H.total_bytes; return SM_OK; }
+  if ((uint64_t)capacity < H.total_bytes) return fail(ctx, SM_ERR_INVALID, "sm_snapshot_save: capacity too small");
+  uint64_t sum = 0;
+  for (int r = 0; r < n; r++) {       // the strips' checksums add up mod 2^64
+    uint64_t part = 0;
+    const int rc = sm_checksum(R[r], &part);
+    if (rc != SM_OK) return ctx->group ? grp_err(ctx, r, rc) : rc;
+    sum += part;
+  }
+  H.checksum = sum;
+  int rc = snap_put_header(R[0], H, (unsigned char*)dst, dev);
+  if (rc != SM_OK) return ctx->group ? grp_err(ctx, 0, rc) : rc;
+  for (int r = 0; r < n; r++) {
+    rc = snap_put_strip(R[r], t[(size_t)r], H, base[(size_t)r], (unsigned char*)dst, dev, d_off[(size_t)r]);
+    if (rc != SM_OK) return ctx->group ? grp_err(ctx, r, rc) : rc;
+  }
+  return SM_OK;
+}
+
+int sm_snapshot_bytes(sm_context* ctx, int64_t* bytes) {
+  if (!bytes) return fail(ctx, SM_ERR_INVALID, "null argument");
+  return snap_save(ctx, bytes, nullptr, 0, false);
+}
+int sm_snapshot_save(sm_context* ctx, void* dst, int64_t capacity, int32_t dst_on_device) {
+  if (!dst) return fail(ctx, SM_ERR_INVALID, "sm_snapshot_save: null destination");
+  return snap_save(ctx, nullptr, dst, capacity, dst_on_device != 0);
+}
+
+// One context's share of a restore: its slice [lo, lo + lcells) of the snapshot's cells, validated and given its pool
+// bases (snap_prepare) before any context's map is written (snap_commit).
+struct SnapIn {
+  DevTmp t;
+  const unsigned long long* off = nullptr;   // device: the slice of the offsets, lcells + 1 of them
+  const SnapRec* rec = nullptr;              // device: the record of index off[0]
+  unsigned long long* base = nullptr;        // device: each column's first pool slot
+  uint64_t need = 0;                         // pool slots (buried sections)
+};
+static int snap_header(sm_context* ctx, const void* src, int64_t bytes, bool dev, SnapHeader& H) {
+  if (!src || bytes < (int64_t)sizeof(H)) return fail(ctx, SM_ERR_INVALID, "snapshot: shorter than its header");
+  if (dev) {
+    CK(cudaSetDevice(ctx->cfg.device));
+    CK(cudaMemcpy(&H, src, sizeof(H), cudaMemcpyDeviceToHost));
+  } else {
+    memcpy(&H, src, sizeof(H));
+  }
+  const char* m = snap_check_header(H, bytes, ctx->d.dimx, ctx->d.dimy, ctx->nsoils);
+  return m ? fail(ctx, SM_ERR_INVALID, m) : SM_OK;
+}
+static int snap_prepare(sm_context* ctx, const SnapHeader& H, const unsigned char* src, bool dev, SnapIn& in) {
+  CK(cudaSetDevice(ctx->cfg.device));
+  CK(cudaStreamSynchronize(ctx->stream));
+  const size_t dimy = (size_t)ctx->d.dimy, L = ctx->lcells;
+  size_t lo;
+  if (H.x0 == ctx->x0 && H.x1 == ctx->x1) lo = 0;
+  else if (H.x0 == 0 && H.x1 == ctx->d.dimx) lo = (size_t)ctx->x0 * dimy;
+  else return fail(ctx, SM_ERR_INVALID, "snapshot: its x-range is neither the whole map nor this context's strip");
+  const unsigned long long* const off = (const unsigned long long*)(src + H.offsets_at);
+  unsigned long long ends[4];          // off[0], off[ncells], off[lo], off[lo + L]
+  const size_t at[4] = {0, (size_t)H.ncells, lo, lo + L};
+  for (int i = 0; i < 4; i++) {
+    if (dev) CK(cudaMemcpy(&ends[i], off + at[i], 8, cudaMemcpyDeviceToHost));
+    else ends[i] = off[at[i]];
+  }
+  if (!snap_check_ends(ends[0], ends[1], ends[2], ends[3], H.nsections))
+    return fail(ctx, SM_ERR_INVALID, "snapshot: offsets do not run from 0 to nsections");
+  const size_t nrec = (size_t)(ends[3] - ends[2]);
+  const SnapRec* const rec = (const SnapRec*)(src + H.records_at) + ends[2];
+  int rc;
+  if (dev) {
+    in.off = off + lo;
+    in.rec = rec;
+  } else {             // a host source: the slice's offsets and records are copied to the device first
+    void* p;
+    if ((rc = snap_alloc(ctx, in.t, (L + 1) * 8, &p)) != SM_OK) return rc;
+    CK(cudaMemcpyAsync(p, off + lo, (L + 1) * 8, cudaMemcpyHostToDevice, ctx->stream));
+    in.off = (const unsigned long long*)p;
+    if ((rc = snap_alloc(ctx, in.t, nrec * sizeof(SnapRec), &p)) != SM_OK) return rc;
+    if (nrec) CK(cudaMemcpyAsync(p, rec, nrec * sizeof(SnapRec), cudaMemcpyHostToDevice, ctx->stream));
+    in.rec = (const SnapRec*)p;
+  }
+  if ((rc = snap_alloc(ctx, in.t, (L + 2) * 8, (void**)&in.base)) != SM_OK) return rc;
+  unsigned int* const d_err = (unsigned int*)(in.base + L + 1);
+  CK(cudaMemsetAsync(d_err, 0, 4, ctx->stream));
+  k_snap_validate<<<ctx->num_sms * 8, 256, 0, ctx->stream>>>(in.off, in.rec, L, ctx->nsoils, in.base, d_err);
+  ctx->launches++;
+  CK(cudaGetLastError());
+  unsigned int err = 0;
+  CK(cudaMemcpyAsync(&err, d_err, 4, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  if (err) return fail(ctx, SM_ERR_INVALID, "snapshot: offsets run backwards or a section's soil type is out of range");
+  if ((rc = snap_scan(ctx, in.t, in.base, L + 1)) != SM_OK) return rc;
+  unsigned long long need = 0;
+  CK(cudaMemcpyAsync(&need, in.base + L, 8, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  in.need = need;
+  if (need >= SM_NIL - L - (4ull << 20)) return fail(ctx, SM_ERR_POOL, "snapshot: more buried sections than pool slots can address");
+  if ((ctx->cfg.pool_capacity > 0 || ctx->nranks > 1) && need > ctx->d.pool_cap)
+    return fail(ctx, SM_ERR_POOL, ctx->nranks > 1 ? "sharded context: pool_capacity is fixed at creation and too small"
+                                                  : "snapshot: pool_capacity too small");
+  return SM_OK;
+}
+static int snap_commit(sm_context* ctx, const SnapHeader& H, const unsigned char* src, SnapIn& in) {
+  CK(cudaSetDevice(ctx->cfg.device));
+  if (ctx->cfg.pool_capacity <= 0 && ctx->nranks == 1) {      // grows as sm_upload_columns does
+    const int rc = alloc_pool(ctx, in.need + (unsigned long long)ctx->lcells + (4ull << 20));
+    if (rc != SM_OK) return rc;
+  }
+  k_snap_unpack<<<ctx->num_sms * 8, 256, 0, ctx->stream>>>(ctx->d, in.off, in.rec, ctx->lcells, in.base);
+  ctx->launches++;
+  CK(cudaGetLastError());
+  float* const dstf[3] = {ctx->d.wfreq, ctx->d.wtrack, ctx->d.windfreq};
+  const size_t w = (size_t)(H.x1 - H.x0);
+  for (int k = 0; k < 3; k++)
+    CK(cudaMemcpy2DAsync(dstf[k] + ctx->x0, 4 * (size_t)ctx->d.dimx,
+                         src + H.freq_at + (size_t)k * 4 * H.ncells + 4 * (size_t)(ctx->x0 - H.x0), 4 * w,
+                         4 * (size_t)(ctx->x1 - ctx->x0), (size_t)ctx->d.dimy, cudaMemcpyDefault, ctx->stream));
+  const int rc = reset_pool_ctl(ctx, in.need);     // synchronises the stream first
+  if (rc != SM_OK) return rc;
+  ctx->cur_kind = -1; ctx->cur_n = 0;              // no batch to resume or flood, as on a fresh context
+  ctx->mesh_valid = false;
+  return SM_OK;
+}
+
+int sm_snapshot_restore(sm_context* ctx, const void* src_, int64_t bytes, int32_t src_on_device) {
+  const bool dev = src_on_device != 0;
+  const unsigned char* const src = (const unsigned char*)src_;
+  const int n = ctx->group ? ctx->group->n : 1;
+  sm_context* const* const R = ctx->group ? ctx->group->rank : &ctx;
+  SnapHeader H;
+  int rc = snap_header(ctx->group ? R[0] : ctx, src, bytes, dev, H);
+  if (rc != SM_OK) return ctx->group ? grp_err(ctx, 0, rc) : rc;
+  if (ctx->group) {
+    if (H.x0 != 0 || H.x1 != ctx->d.dimx) return fail(ctx, SM_ERR_INVALID, "snapshot: a group restores whole-map snapshots only");
+    if ((rc = grp_settle(ctx)) != SM_OK) return rc;
+  }
+  std::vector<SnapIn> in((size_t)n);
+  for (int r = 0; r < n; r++)            // every rank validates its slice before any rank writes
+    if ((rc = snap_prepare(R[r], H, src, dev, in[(size_t)r])) != SM_OK) return ctx->group ? grp_err(ctx, r, rc) : rc;
+  if (ctx->group) { ctx->group->dirty = true; ctx->cur_kind = -1; ctx->cur_n = 0; }
+  for (int r = 0; r < n; r++)
+    if ((rc = snap_commit(R[r], H, src, in[(size_t)r])) != SM_OK) return ctx->group ? grp_err(ctx, r, rc) : rc;
+  // the map now holds what the snapshot describes; its checksum is checked where this context holds all it covers
+  if (ctx->group || (H.x0 == ctx->x0 && H.x1 == ctx->x1)) {
+    uint64_t sum = 0, part = 0;
+    for (int r = 0; r < n; r++) {
+      if ((rc = sm_checksum(R[r], &part)) != SM_OK) return ctx->group ? grp_err(ctx, r, rc) : rc;
+      sum += part;
+    }
+    if (sum != H.checksum) return fail(ctx, SM_ERR_INVALID, "snapshot: the restored columns do not match the header's checksum");
+  }
   return SM_OK;
 }
 

@@ -14,6 +14,7 @@ import numpy as np
 from . import capi, presets
 
 _libc = None
+_draws = 0       # rand() draws since the last srand (Simulation.save stores it, Simulation.load replays it)
 
 
 def _c():
@@ -26,12 +27,21 @@ def _c():
 
 
 def srand(seed):
+    global _draws
     _c().srand(int(seed) & 0xFFFFFFFF)
+    _draws = 0
+
+
+def draws():
+    """rand() draws made by spawn_list since the last srand"""
+    return _draws
 
 
 def spawn_list(n, dimx, dimy):
     """n (x, y) spawn positions = n constructor calls' worth of rand() draws."""
+    global _draws
     lc = _c()
+    _draws += 2 * n
     out = np.empty((n, 2), np.float32)
     for i in range(n):
         y = lc.rand() % dimy
@@ -57,6 +67,7 @@ class Simulation:
         self.scale = int(w["scale"])
         self.seed = int(seed)
         srand(self.seed)                                   # SoilMachine.cpp:41
+        self.soil = str(soil)
         self.ctx = capi.Context(self.dimx, self.dimy, self.scale, device=device,
                                 pool_capacity=pool_capacity, max_particles=max_particles, gpus=gpus, devices=devices,
                                 budget=budget, cell_budget=cell_budget)
@@ -90,6 +101,33 @@ class Simulation:
         if nwater:
             self.ctx.frequency_update()
         return ws, ds
+
+    def save(self, path):
+        """Write the simulation to `path`: the snapshot of the map (columns and frequency arrays), the soil preset, the
+        seed and the rand() draws made since srand.  A Simulation.load of the file continues the run with the same
+        spawn lists.  Not saved: the volume factor, the wind lattice, budgets (snapshot.py lists the rest)."""
+        with open(path, "wb") as f:
+            np.savez(f, snapshot=self.ctx.snapshot(), soil=np.array(self.soil), seed=np.int64(self.seed),
+                     draws=np.int64(_draws))
+
+    @classmethod
+    def load(cls, path, device=0, gpus=1, devices=None, **kw):
+        """A Simulation from a file of save(), on any number of GPUs (gpus / devices as in __init__, other keyword
+        arguments too): the map is restored from the snapshot, rand() is re-seeded and the saved number of draws is
+        discarded, so later frames draw the spawn lists the uninterrupted run would have drawn."""
+        global _draws
+        with np.load(path) as z:
+            buf, soil, seed, n = z["snapshot"], str(z["soil"]), int(z["seed"]), int(z["draws"])
+        from . import snapshot
+        h = snapshot.header(buf)
+        sim = cls(soil, seed=seed, dimx=h["dimx"], dimy=h["dimy"], device=device, gpus=gpus, devices=devices, **kw)
+        sim.ctx.restore(buf)
+        srand(seed)
+        lc = _c()
+        for _ in range(n):
+            lc.rand()
+        _draws = n
+        return sim
 
     def close(self):
         self.ctx.close()

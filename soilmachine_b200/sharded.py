@@ -9,7 +9,7 @@ DistShard      - one rank per process / GPU under torch.distributed: peer blobs 
 """
 import ctypes as C
 import numpy as np
-from . import capi
+from . import capi, snapshot as snap
 
 
 def split_columns(cols, dimx, dimy, x0, x1):
@@ -43,6 +43,15 @@ def merge_frequency(parts, ranges, dimx, dimy):
             m[:, x0:x1] = p[k].reshape(dimy, dimx)[:, x0:x1]
         out[k] = m.reshape(-1)
     return out
+
+
+def check_restored(buf, checksums):
+    """A rank restoring its slice of a whole-map snapshot cannot check the header's checksum alone: the ranks'
+    checksums after the restore must add up (mod 2^64) to it."""
+    h = snap.header(buf)
+    if h["x0"] == 0 and h["x1"] == h["dimx"] and sum(checksums) % (1 << 64) != h["checksum"]:
+        raise capi.SoilMachineError(capi.SM_ERR_INVALID, "snapshot: the restored columns do not match the header's "
+                                                         "checksum")
 
 
 def sum_stats(stats):
@@ -85,6 +94,19 @@ class VirtualShards:
 
     def download_columns(self):
         return merge_columns([c.download_columns() for c in self.ctx])
+
+    def snapshot(self):
+        """the whole-map snapshot: every rank saves its strip, the strips are joined"""
+        self.sync()
+        return np.frombuffer(snap.join([c.snapshot() for c in self.ctx]), np.uint8)
+
+    def restore(self, buf):
+        """every rank restores its slice of a whole-map snapshot (host bytes); the ranks' checksums are then compared
+        with the header's"""
+        self.sync()
+        for c in self.ctx:
+            c.restore(buf)
+        check_restored(buf, [c.checksum() for c in self.ctx])
 
     def heights(self):
         return np.concatenate([c.heights() for c in self.ctx], axis=0)
@@ -216,6 +238,24 @@ class DistShard:
         dist.all_gather_object(blobs, mine)
         self.ctx.peer_attach([capi.PeerBlob.from_buffer_copy(b) for b in blobs], use_ipc=True)
         dist.barrier()
+
+    def snapshot(self):
+        """the whole-map snapshot on every rank: all ranks must call it (each saves its strip, the strips are
+        gathered and joined)"""
+        self._settle()
+        strips = [None] * self.nranks
+        self.dist.all_gather_object(strips, self.ctx.snapshot().tobytes())
+        return np.frombuffer(snap.join(strips), np.uint8)
+
+    def restore(self, buf):
+        """every rank restores its slice of the same whole-map snapshot (or a strip snapshot of its own range); all
+        ranks must call it.  The ranks' checksums are then compared with a whole-map snapshot's header."""
+        self._settle()
+        self.ctx.restore(buf)
+        sums = [None] * self.nranks
+        self.dist.all_gather_object(sums, self.ctx.checksum())
+        self.dist.barrier()
+        check_restored(buf, sums)
 
     def run(self, kind, d_xy, n, max_sweeps=0):
         """launch this rank's sweep kernel (all ranks must call it), wait, return local stats"""
