@@ -213,6 +213,13 @@ class Layermap {
     pool.unget(E);
   }
   double remove(ivec2 p, double h) { double d; touch(); ck(sm_cell_remove(ctx, p.x, p.y, h, &d)); return d; }   // :310
+  // add() / a full strip over remove() on every cell in one call (sm_apply_layer): delta[x*dim.y + y] > 0 deposits that
+  // much of `type`, < 0 strips that much height, +-0.0 leaves the cell alone; leftover (may be null) gets the height each
+  // strip could not take.  All or nothing: a refused raster throws with the map unchanged.
+  void apply(const double* delta, SurfType type, double* leftover = nullptr) {
+    touch();
+    ck(sm_apply_layer(ctx, delta, (int32_t)type, leftover, 0, 0, nullptr));
+  }
 
   // ---- meshing (layermap.h:443-555) --------------------------------------------------------------------------
   // The renderer's vertex pool is outside the boundary; what crosses it is the vertex data.  update(vp) meshes

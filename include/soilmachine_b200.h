@@ -106,6 +106,7 @@ int sm_sync(sm_context* ctx);
  * touch the map until it returns.  On a rank that is not the issuer these calls return SM_ERR_INVALID, so that a call
  * made on every rank in lockstep, as the batches are, cannot run several times over the same map.  The single-cell
  * calls that change the map return SM_ERR_INVALID on a sharded context; a group (sm_create_group) offers them.
+ * sm_apply_layer works on a rank's own strip (same precondition).
  * sm_peer_attach with use_ipc = 0 enables peer access to a blob's device when it differs from the context's. */
 #define SM_PEER_ARRAYS 23
 #define SM_PEER_SLOTS 24
@@ -238,6 +239,45 @@ int sm_checksum(sm_context* ctx, uint64_t* checksum);
 int sm_snapshot_bytes(sm_context* ctx, int64_t* bytes);
 int sm_snapshot_save(sm_context* ctx, void* dst, int64_t capacity, int32_t dst_on_device);
 int sm_snapshot_restore(sm_context* ctx, const void* src, int64_t bytes, int32_t src_on_device);
+
+/* ---- layer rasters: deposit or strip one soil type on every cell in one call (DESIGN.md section 11) ------------------
+ * delta: one f64 per cell, cell order (x - x0)*dimy + y - the whole map on a plain context and on a group, the rank's
+ * strip [x0, x1) on a rank of a sharded map.  type: one soil index, 0 <= type < nsoils.  For every cell:
+ *   delta > 0   exactly sm_cell_add(x, y, delta, type), i.e. Layermap::add(pos, new sec(delta, type)) (layermap.h:230-307),
+ *               the Air case included: the new section goes under the standing water, the water back on top;
+ *   delta < 0   strips h = -delta with the reference's own Layermap::remove (layermap.h:310-339):
+ *                 left = h; while (left > 0 && dat[pos] != NULL) { empty_top = dat[pos]->size <= 0;
+ *                                                                  r = remove(pos, left); if (!empty_top) left = r; }
+ *               a zero-size top is popped without using up height; leftover[cell] = left, non-zero only where the
+ *               column ran empty (one remove() call would stop at the first section boundary);
+ *   +-0.0       the cell is untouched.
+ * Each cell changes its own column only and pool slots never influence values, so the result does not depend on the
+ * order the cells run in: it is the result of those calls made cell by cell.  Frequency arrays, budgets, per-cell maps
+ * and hydrology maps are not touched; the mesh is left as sm_cell_add leaves it (sm_mesh_update recomputes it); an open
+ * batch is treated as by sm_cell_add.
+ * All or nothing: nothing is written unless every entry is finite, type is in range (SM_ERR_INVALID otherwise) and the
+ * pool can serve every section the raster pushes - counted exactly first: 0 on an empty column or an equal-type top, 1
+ * for an ordinary push, 0 to 2 on an Air top - from the slots it can hand out now (SM_ERR_POOL otherwise; the pool is
+ * not grown).  A refused call leaves the map as it was.
+ * on_device != 0: delta and leftover are device pointers on the context's device (rank 0's for a group); otherwise host
+ * memory, and the raster is staged through 8 B per cell of device memory (16 B with leftover).  leftover may be NULL.
+ * check_only != 0: run the check alone and fill stats (the all-or-nothing decision of a map sharded over processes:
+ * every rank checks, the ranks agree, then every rank applies).  stats may be NULL; on SM_ERR_POOL it still holds the
+ * counts.
+ * Rank of a sharded map: allowed (its columns and their buried sections live in its own pool; no peer access), with the
+ * precondition of the read-only views: every rank's earlier work has completed (sm_sync on every rank, then a host
+ * barrier).  The single-cell calls stay refused there.  Group: every rank checks its slice of the raster (a device
+ * raster is copied to the other ranks' devices), any refusal refuses the whole call, then every rank applies
+ * concurrently; the stats are summed, device_ms is the slowest rank's. */
+typedef struct sm_layer_stats {
+  int64_t cells;       /* cells with delta != 0 */
+  int64_t pushed;      /* sections the raster pushes (what the pool had to serve) */
+  int64_t free_slots;  /* slots the pool could hand out when the call began */
+  int64_t emptied;     /* columns stripped to empty (leftover > 0) */
+  double device_ms;    /* CUDA-event time of the check and apply kernels */
+} sm_layer_stats;
+int sm_apply_layer(sm_context* ctx, const double* delta, int32_t type, double* leftover, int32_t on_device,
+                   int32_t check_only, sm_layer_stats* stats);
 
 /* WaterParticle::frequency/track, WindParticle::frequency (water.h:345-346, wind.h:48).
  * Any pointer may be NULL. */

@@ -40,6 +40,7 @@ SYMBOLS = [
     "sm_lbm_step", "sm_lbm_get", "sm_lbm_advect", "sm_wind_use_lbm",
     "sm_create_group", "sm_group_size", "sm_group_rank", "sm_group_layout",
     "sm_snapshot_bytes", "sm_snapshot_save", "sm_snapshot_restore",
+    "sm_apply_layer",
 ]
 
 
@@ -79,6 +80,14 @@ class HydroBudget(C.Structure):
     _fields_ = [(k, C.c_double) for k in (
         "flood_sediment", "flood_cascade_net", "flood_water", "seeped", "to_particles", "transfer_net",
         "nested_eroded", "nested_deposited", "nested_cascade_net", "nested_discarded", "nested_clamped")]
+
+    def asdict(self):
+        return {k: getattr(self, k) for k, _ in self._fields_}
+
+
+class LayerStats(C.Structure):
+    _fields_ = [("cells", C.c_int64), ("pushed", C.c_int64), ("free_slots", C.c_int64), ("emptied", C.c_int64),
+                ("device_ms", C.c_double)]
 
     def asdict(self):
         return {k: getattr(self, k) for k, _ in self._fields_}
@@ -338,6 +347,32 @@ class Context:
             return
         a = np.frombuffer(memoryview(buf), np.uint8)
         self._ck_strict(self.lib.sm_snapshot_restore(self.h, a.ctypes.data_as(C.c_void_p), C.c_int64(a.size), 0))
+
+    # ---- layer rasters ---------------------------------------------------------------------------------------------
+    def apply_layer(self, delta, type, leftover=False, check=False):
+        """sm_apply_layer: deposit (delta > 0) or strip (delta < 0) soil `type` on every cell in one call.  delta is a
+        float64 array of shape (x1 - x0, dimy) - the whole map, or this rank's strip of a sharded map - or a device
+        pointer from device_alloc holding that many doubles.  leftover=True (host raster) returns the leftovers as an
+        array of that shape; with a device raster, leftover may be a device pointer to write them to.  check=True runs
+        the all-or-nothing check alone.  Returns (LayerStats, leftovers or None); a refusal raises with the map
+        unchanged (SM_ERR_POOL included)."""
+        st = LayerStats()
+        if isinstance(delta, np.ndarray):
+            d = np.ascontiguousarray(delta, np.float64)
+            if d.shape != (self.x1 - self.x0, self.dimy):
+                raise SoilMachineError(SM_ERR_INVALID, "apply_layer: the raster has shape %s, the map (%d, %d)"
+                                       % (d.shape, self.x1 - self.x0, self.dimy))
+            left = np.zeros_like(d) if leftover else None
+            self._ck_strict(self.lib.sm_apply_layer(self.h, _p(d, C.c_double), int(type), _p(left, C.c_double), 0,
+                                                    int(bool(check)), C.byref(st)))
+            return st, left
+        if leftover is True:
+            raise SoilMachineError(SM_ERR_INVALID, "apply_layer: a device raster writes leftovers to a device pointer")
+        d = C.c_void_p(delta.value if isinstance(delta, C.c_void_p) else delta)
+        left = None if leftover is False or leftover is None else \
+            C.c_void_p(leftover.value if isinstance(leftover, C.c_void_p) else leftover)
+        self._ck_strict(self.lib.sm_apply_layer(self.h, d, int(type), left, 1, int(bool(check)), C.byref(st)))
+        return st, left
 
     def set_soil_colors(self, rgba):
         rgba = np.ascontiguousarray(rgba, np.float32).reshape(-1, 4)

@@ -21,6 +21,7 @@
 #include "sm_hydro.cuh"
 #include "sm_lbm.cuh"
 #include "sm_snap.cuh"
+#include "sm_layer.cuh"
 #include <cub/device/device_scan.cuh>
 
 #define KIND_WATER 0
@@ -900,6 +901,59 @@ __global__ void __launch_bounds__(256) k_snap_unpack(DevCtx c, const unsigned lo
                                                      const unsigned long long* __restrict__ base) {
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < cells; i += (size_t)gridDim.x * blockDim.x)
     snap_unpack_cell((const uint64_t*)off, rec, i, (uint32_t)base[i], c.top[i], c.pool);
+}
+
+// ---- layer rasters (sm_layer.cuh): one thread per cell of this context's strip, pool phase 0 as k_cell_op ------------
+// the block's sum of v into *out
+__device__ __forceinline__ void block_add_u64(unsigned long long v, unsigned long long* out) {
+  __shared__ unsigned long long sh[8];
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(0xFFFFFFFFu, v, o);
+  if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = v;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    unsigned long long s = 0;
+    for (int w = 0; w < (int)(blockDim.x >> 5); w++) s += sh[w];
+    if (s) atomicAdd(out, s);
+  }
+}
+// before any write: out[0] += pool slots the raster will allocate, out[1] += cells it touches, out[2] |= 1 when an
+// entry is not finite or the type is out of range.  Reads the raster and, where delta > 0, the top record (and on an Air
+// top the record underneath).
+__global__ void __launch_bounds__(256) k_layer_check(DevCtx c, const double* __restrict__ delta, size_t cells, int type,
+                                                     unsigned long long* __restrict__ out) {
+  DevAccess a(c, nullptr, 0u);
+  unsigned long long pushed = 0, touched = 0;
+  bool bad = false;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < cells; i += (size_t)gridDim.x * blockDim.x) {
+    const double d = delta[i];
+    if (!layer_input_ok(d, type, c.nsoils)) { bad = true; continue; }
+    touched += d != 0.0;
+    if (d > 0) pushed += layer_pushes(a, c.top[i], d, (uint32_t)type);
+  }
+  if (bad) atomicOr(&out[2], 1ull);
+  block_add_u64(pushed, &out[0]);
+  __syncthreads();
+  block_add_u64(touched, &out[1]);
+}
+// every cell with delta != 0: read the top record, apply, write it back; frees to ring 0, allocations from ring 1 or the
+// bump counter.  leftover (nullable) gets every cell's leftover, *emptied += cells whose leftover is > 0.
+__global__ void __launch_bounds__(256) k_layer_apply(DevCtx c, const double* __restrict__ delta, size_t cells,
+                                                     uint32_t type, double* __restrict__ leftover,
+                                                     unsigned long long* __restrict__ emptied) {
+  DevAccess a(c, nullptr, 0u);
+  unsigned long long n = 0;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < cells; i += (size_t)gridDim.x * blockDim.x) {
+    const double d = delta[i];
+    double left = 0.0;
+    if (d != 0.0) {
+      Sec32 r = c.top[i];
+      left = layer_apply_cell(a, r, d, type);
+      c.top[i] = r;
+    }
+    if (leftover) leftover[i] = left;
+    n += left > 0;
+  }
+  block_add_u64(n, emptied);
 }
 
 // Layermap::initialize, layermap.h:163-216: one thread per cell replays add() for every layer
@@ -3284,6 +3338,154 @@ int sm_snapshot_restore(sm_context* ctx, const void* src_, int64_t bytes, int32_
     }
     if (sum != H.checksum) return fail(ctx, SM_ERR_INVALID, "snapshot: the restored columns do not match the header's checksum");
   }
+  return SM_OK;
+}
+
+// ---- layer rasters (sm_layer.cuh, DESIGN.md section 11) ----------------------------------------------------------
+// One context's share of sm_apply_layer: its strip of the raster, checked and counted (layer_check) before any context's
+// map is written (layer_launch, layer_finish).
+struct LayerIn {
+  DevTmp t;
+  const double* delta = nullptr;             // device: the strip's raster
+  double* left = nullptr;                    // device: where k_layer_apply writes the leftovers (null: nowhere)
+  unsigned long long* d_out = nullptr;       // device: pushed, touched, error, emptied
+  cudaEvent_t e0 = nullptr, e1 = nullptr;
+  sm_layer_stats st = {};
+  ~LayerIn() {
+    if (e0) cudaEventDestroy(e0);
+    if (e1) cudaEventDestroy(e1);
+  }
+};
+// src: the strip's raster, on the host or (dev) on this context's device; src_dev0: a raster on `dev0` (a group's rank 0)
+// that is copied over after ev0 on that device's stream.  want_left: k_layer_apply writes leftovers (into `left_dev`
+// when given, a device buffer on this context's device, else into a staging buffer).
+static int layer_check(sm_context* ctx, const double* src, bool dev, const double* src_dev0, int dev0, cudaEvent_t ev0,
+                       int32_t type, bool want_left, double* left_dev, LayerIn& in) {
+  if (ctx->nsoils < 1) return fail(ctx, SM_ERR_INVALID, "soil table not set");
+  if (type < 0 || type >= ctx->nsoils) return fail(ctx, SM_ERR_INVALID, "sm_apply_layer: type out of range");
+  CK(cudaSetDevice(ctx->cfg.device));
+  const size_t L = ctx->lcells;
+  int rc;
+  if ((rc = snap_alloc(ctx, in.t, 4 * 8, (void**)&in.d_out)) != SM_OK) return rc;
+  CK(cudaMemsetAsync(in.d_out, 0, 4 * 8, ctx->stream));
+  if (src_dev0) {
+    void* p;
+    if ((rc = snap_alloc(ctx, in.t, L * 8, &p)) != SM_OK) return rc;
+    CK(cudaStreamWaitEvent(ctx->stream, ev0, 0));
+    CK(cudaMemcpyPeerAsync(p, ctx->cfg.device, src_dev0, dev0, L * 8, ctx->stream));
+    in.delta = (const double*)p;
+  } else if (!dev) {            // a host raster is staged: L x 8 bytes of device memory
+    void* p;
+    if ((rc = snap_alloc(ctx, in.t, L * 8, &p)) != SM_OK) return rc;
+    CK(cudaMemcpyAsync(p, src, L * 8, cudaMemcpyHostToDevice, ctx->stream));
+    in.delta = (const double*)p;
+  } else {
+    in.delta = src;
+  }
+  if (want_left) {
+    if (left_dev) in.left = left_dev;
+    else if ((rc = snap_alloc(ctx, in.t, L * 8, (void**)&in.left)) != SM_OK) return rc;
+  }
+  CK(cudaEventCreate(&in.e0));
+  CK(cudaEventCreate(&in.e1));
+  CK(cudaEventRecord(in.e0, ctx->stream));
+  k_layer_check<<<ctx->num_sms * 8, 256, 0, ctx->stream>>>(ctx->d, in.delta, L, type, in.d_out);
+  ctx->launches++;
+  CK(cudaGetLastError());
+  CK(cudaEventRecord(in.e1, ctx->stream));
+  unsigned long long out[3];
+  RunCtl h;                     // the pool's state: bump counter and rings, as the last call left them
+  CK(cudaMemcpyAsync(out, in.d_out, 3 * 8, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaMemcpyAsync(&h.bump, &ctx->d.ctl->bump, sizeof(h.bump) + sizeof(h.ring), cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  float ms = 0.f;
+  CK(cudaEventElapsedTime(&ms, in.e0, in.e1));
+  const unsigned long long cap = ctx->d.pool_cap;
+  in.st.cells = (int64_t)out[1];
+  in.st.pushed = (int64_t)out[0];
+  in.st.free_slots = (int64_t)((h.ring[1].tail - h.ring[1].head) + (cap - std::min(h.bump, cap)));
+  in.st.device_ms = ms;
+  if (out[2]) return fail(ctx, SM_ERR_INVALID, "sm_apply_layer: a raster entry is not finite");
+  if (in.st.pushed > in.st.free_slots)
+    return fail(ctx, SM_ERR_POOL, "sm_apply_layer: the raster pushes more sections than the pool has free slots");
+  return SM_OK;
+}
+// the apply kernel of a checked strip, left in flight
+static int layer_launch(sm_context* ctx, uint32_t type, LayerIn& in) {
+  CK(cudaSetDevice(ctx->cfg.device));
+  CK(cudaEventRecord(in.e0, ctx->stream));
+  k_layer_apply<<<ctx->num_sms * 8, 256, 0, ctx->stream>>>(ctx->d, in.delta, ctx->lcells, type, in.left, in.d_out + 3);
+  ctx->launches++;
+  CK(cudaGetLastError());
+  CK(cudaEventRecord(in.e1, ctx->stream));
+  return SM_OK;
+}
+// wait for the apply; left_host: copy the leftovers there; left_dev0: copy them to that buffer on device dev0
+static int layer_finish(sm_context* ctx, LayerIn& in, double* left_host, double* left_dev0, int dev0) {
+  CK(cudaSetDevice(ctx->cfg.device));
+  const size_t L = ctx->lcells;
+  unsigned long long emptied = 0;
+  CK(cudaMemcpyAsync(&emptied, in.d_out + 3, 8, cudaMemcpyDeviceToHost, ctx->stream));
+  if (left_host) CK(cudaMemcpyAsync(left_host, in.left, L * 8, cudaMemcpyDeviceToHost, ctx->stream));
+  if (left_dev0) CK(cudaMemcpyPeerAsync(left_dev0, dev0, in.left, ctx->cfg.device, L * 8, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  float ms = 0.f;
+  CK(cudaEventElapsedTime(&ms, in.e0, in.e1));
+  in.st.emptied = (int64_t)emptied;
+  in.st.device_ms += ms;
+  return SM_OK;
+}
+
+int sm_apply_layer(sm_context* ctx, const double* delta, int32_t type, double* leftover, int32_t on_device,
+                   int32_t check_only, sm_layer_stats* stats) {
+  if (!delta) return fail(ctx, SM_ERR_INVALID, "sm_apply_layer: null raster");
+  const bool dev = on_device != 0, want_left = leftover != nullptr && !check_only;
+  const int n = ctx->group ? ctx->group->n : 1;
+  sm_context* const* const R = ctx->group ? ctx->group->rank : &ctx;
+  int rc;
+  if (ctx->group && (rc = grp_settle(ctx)) != SM_OK) return rc;
+  sm_context* const c0 = R[0];
+  if (ctx->group && dev) {      // the ranks' slices of a device raster are copied from rank 0's device after its stream
+    CK(cudaSetDevice(c0->cfg.device));
+    CK(cudaEventRecord(ctx->group->ev, c0->stream));
+  }
+  std::vector<LayerIn> in((size_t)n);
+  sm_layer_stats tot = {};
+  auto add = [&](const sm_layer_stats& s) {
+    tot.cells += s.cells; tot.pushed += s.pushed; tot.free_slots += s.free_slots; tot.emptied += s.emptied;
+    tot.device_ms = std::max(tot.device_ms, s.device_ms);
+  };
+  int bad = -1, bad_rc = SM_OK;
+  for (int r = 0; r < n; r++) {     // every rank checks its strip before any rank writes
+    sm_context* const c = R[r];
+    const size_t off = ctx->group ? (size_t)c->x0 * ctx->d.dimy : 0;
+    const bool peer = ctx->group && dev && r > 0;
+    double* const ldev = (want_left && dev && !peer) ? leftover + off : nullptr;
+    rc = layer_check(c, peer ? nullptr : delta + off, dev, peer ? delta + off : nullptr, c0->cfg.device,
+                     ctx->group ? ctx->group->ev : nullptr, type, want_left, ldev, in[(size_t)r]);
+    add(in[(size_t)r].st);
+    if (rc != SM_OK && bad < 0) { bad = r; bad_rc = rc; }
+    if (rc != SM_OK && rc != SM_ERR_POOL) break;     // the other ranks' counts only matter for a pool refusal
+  }
+  if (bad >= 0 || check_only) {
+    if (stats) *stats = tot;
+    if (bad >= 0) return ctx->group ? grp_err(ctx, bad, bad_rc) : bad_rc;
+    return SM_OK;
+  }
+  if (ctx->group) ctx->group->dirty = true;
+  for (int r = 0; r < n; r++)       // every rank's apply is in flight before any is waited for
+    if ((rc = layer_launch(R[r], (uint32_t)type, in[(size_t)r])) != SM_OK) return ctx->group ? grp_err(ctx, r, rc) : rc;
+  tot = {};
+  for (int r = 0; r < n; r++) {
+    sm_context* const c = R[r];
+    const size_t off = ctx->group ? (size_t)c->x0 * ctx->d.dimy : 0;
+    const bool peer = ctx->group && dev && r > 0;
+    rc = layer_finish(c, in[(size_t)r], want_left && !dev ? leftover + off : nullptr,
+                      want_left && peer ? leftover + off : nullptr, c0->cfg.device);
+    if (rc != SM_OK) return ctx->group ? grp_err(ctx, r, rc) : rc;
+    add(in[(size_t)r].st);
+  }
+  if (stats) *stats = tot;
   return SM_OK;
 }
 

@@ -102,6 +102,13 @@ class Simulation:
             self.ctx.frequency_update()
         return ws, ds
 
+    def apply_layer(self, delta, soil, leftover=False):
+        """Deposit (delta > 0) or strip (delta < 0) one soil on every cell (capi.Context.apply_layer, sm_apply_layer):
+        delta is a (dimx, dimy) float64 raster, soil a name of the preset's soil table or an index.  Returns the stats
+        and, with leftover=True, the height each strip could not take."""
+        typ = self.preset["soil_names"].index(soil) if isinstance(soil, str) else int(soil)
+        return self.ctx.apply_layer(delta, typ, leftover=leftover)
+
     def save(self, path):
         """Write the simulation to `path`: the snapshot of the map (columns and frequency arrays), the soil preset, the
         seed and the rand() draws made since srand.  A Simulation.load of the file continues the run with the same

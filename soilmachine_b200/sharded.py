@@ -54,6 +54,22 @@ def check_restored(buf, checksums):
                                                          "checksum")
 
 
+def sum_layer_stats(stats):
+    tot = capi.LayerStats()
+    for f, _ in capi.LayerStats._fields_:
+        vals = [getattr(s, f) for s in stats]
+        setattr(tot, f, max(vals) if f == "device_ms" else sum(vals))
+    return tot
+
+
+def _layer_check(ctx, delta, type):
+    """one rank's check pass: (accepted, stats, refusal)"""
+    try:
+        return True, ctx.apply_layer(delta, type, check=True)[0], None
+    except capi.SoilMachineError as e:
+        return False, None, e
+
+
 def sum_stats(stats):
     tot = capi.Stats()
     for f, _ in capi.Stats._fields_:
@@ -107,6 +123,19 @@ class VirtualShards:
         for c in self.ctx:
             c.restore(buf)
         check_restored(buf, [c.checksum() for c in self.ctx])
+
+    def apply_layer(self, delta, type, leftover=False):
+        """sm_apply_layer over the whole map, all or nothing: every rank checks its strip of the (dimx, dimy) raster,
+        and only when every rank accepts does every rank apply it.  Returns (summed stats, leftovers or None)."""
+        delta = np.ascontiguousarray(delta, np.float64)
+        self.sync()
+        for c in self.ctx:
+            ok, _, err = _layer_check(c, delta[c.x0:c.x1], type)
+            if not ok:
+                raise err
+        out = [c.apply_layer(delta[c.x0:c.x1], type, leftover=leftover) for c in self.ctx]
+        self.sync()
+        return sum_layer_stats([o[0] for o in out]), (np.concatenate([o[1] for o in out]) if leftover else None)
 
     def heights(self):
         return np.concatenate([c.heights() for c in self.ctx], axis=0)
@@ -256,6 +285,21 @@ class DistShard:
         self.dist.all_gather_object(sums, self.ctx.checksum())
         self.dist.barrier()
         check_restored(buf, sums)
+
+    def apply_layer(self, delta, type, leftover=False):
+        """sm_apply_layer over the whole map, all or nothing; all ranks must call it, each with its own strip
+        (x1 - x0, dimy) of the raster.  Every rank checks, the outcomes are gathered, then every rank applies.  Returns
+        this rank's (stats, leftovers or None); a refusal on any rank raises on every rank with no rank written."""
+        self._settle()
+        ok, _, err = _layer_check(self.ctx, delta, type)
+        oks = [None] * self.nranks
+        self.dist.all_gather_object(oks, ok)
+        if not all(oks):
+            raise err if err is not None else capi.SoilMachineError(
+                capi.SM_ERR_INVALID, "apply_layer: refused on another rank")
+        out = self.ctx.apply_layer(delta, type, leftover=leftover)
+        self._settle()
+        return out
 
     def run(self, kind, d_xy, n, max_sweeps=0):
         """launch this rank's sweep kernel (all ranks must call it), wait, return local stats"""
