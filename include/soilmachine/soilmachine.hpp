@@ -220,6 +220,15 @@ class Layermap {
     touch();
     ck(sm_apply_layer(ctx, delta, (int32_t)type, leftover, 0, 0, nullptr));
   }
+  // Particle::cascade (particle.h:24-101) at every cell, pass after pass in sm_relax's phase order, until a pass
+  // changes nothing or max_passes passes have run.  A refused call (transferloop outside 0..3, max_passes < 1) throws
+  // with the map unchanged.
+  sm_relax_stats relax(int max_passes, int transferloop = 0) {
+    sm_relax_stats st = {};
+    touch();
+    ck(sm_relax(ctx, max_passes, transferloop, &st));
+    return st;
+  }
 
   // ---- meshing (layermap.h:443-555) --------------------------------------------------------------------------
   // The renderer's vertex pool is outside the boundary; what crosses it is the vertex data.  update(vp) meshes

@@ -106,7 +106,8 @@ int sm_sync(sm_context* ctx);
  * touch the map until it returns.  On a rank that is not the issuer these calls return SM_ERR_INVALID, so that a call
  * made on every rank in lockstep, as the batches are, cannot run several times over the same map.  The single-cell
  * calls that change the map return SM_ERR_INVALID on a sharded context; a group (sm_create_group) offers them.
- * sm_apply_layer works on a rank's own strip (same precondition).
+ * sm_apply_layer works on a rank's own strip (same precondition).  sm_relax returns SM_ERR_INVALID on a sharded context:
+ * each of its phases needs every rank's previous phase, a barrier across processes per phase; a group offers it.
  * sm_peer_attach with use_ipc = 0 enables peer access to a blob's device when it differs from the context's. */
 #define SM_PEER_ARRAYS 23
 #define SM_PEER_SLOTS 24
@@ -278,6 +279,47 @@ typedef struct sm_layer_stats {
 } sm_layer_stats;
 int sm_apply_layer(sm_context* ctx, const double* delta, int32_t type, double* leftover, int32_t on_device,
                    int32_t check_only, sm_layer_stats* stats);
+
+/* ---- slope relaxation: Particle::cascade at every cell until the slopes are stable (DESIGN.md section 12) -----------
+ * Runs up to max_passes passes of the reference's Particle::cascade(vec2(x, y), map, vp, transferloop)
+ * (particle.h:24-101) over every cell, in this order:
+ *   R = 1 + transferloop                  // footprint radius of one cascade call, re-cascades included
+ *   P = 2R + 1                            // phase period: 3, 5, 7, 9 for transferloop 0..3
+ *   for pass in 1..max_passes:
+ *     for p in 0 .. P*P-1:                // phase p = (px, py) = (p / P, p % P)
+ *       for x = px; x < dimx; x += P:     // x-major inside a phase
+ *         for y = py; y < dimy; y += P:
+ *           Particle::cascade(vec2(x, y), map, vp, transferloop)
+ * A cascade at c reads and writes only the columns within Chebyshev distance R of c, two cells of one phase are at
+ * least P = 2R + 1 apart and pool slot numbers never influence values, so the cells of a phase commute exactly: the
+ * device runs each phase at once, and the result is the result of the calls above, cell by cell.
+ * transferloop: 0..3 (the reference's water particles use 0, its wind particles 1); max_passes >= 1; SM_ERR_INVALID
+ * otherwise, with the map unchanged.
+ * A visit that cannot change anything is skipped: a cascade call is a function of the columns within R, the soil table
+ * and SCALE, so a cell is visited only when a column within R of it changed since its previous visit in this call, or
+ * that visit changed something (every cell is visited in the first pass).  A column changed when its top record's
+ * bytes differ before and after; settling == 0 and transfers col_add ignores change nothing.  The skipped visits are
+ * exact no-ops: the result is the same as visiting every cell.
+ * A pass that changes no column leaves nothing to visit, so the call stops there: the map then equals the result of
+ * exactly max_passes passes.  stats->passes = passes run, stats->stable = 1 when the last pass changed nothing.  The
+ * passes need not converge (with SCALE > 80 and settling near 1 a transfer can overshoot and oscillate), hence the cap.
+ * Frequency arrays, budgets, per-cell budget maps and hydrology maps are not touched; the mesh is left as
+ * sm_cell_cascade leaves it (sm_mesh_update recomputes it); an open batch is treated as by sm_cell_add.
+ * Pool: a section the pool cannot serve is dropped, as the reference does (layermap.h:92-95); the call finishes the
+ * phase in which that happened, stops and returns SM_ERR_POOL with the partial stats (which cells lose the race for
+ * the last slots is not pinned).  Slots freed by one phase are reused by the next.
+ * Group: every rank runs each phase on the phase cells of its strip (global coordinates, the one-context order) and
+ * reaches its neighbours' columns, pools and stale bits through the peer pointers; the counts are summed, device_ms
+ * is the slowest rank's.  Rank of a sharded map: SM_ERR_INVALID (see sm_peer_attach above).  stats may be NULL. */
+typedef struct sm_relax_stats {
+  int64_t passes;      /* passes run */
+  int64_t stable;      /* 1: the last pass changed no column */
+  int64_t visits;      /* cascade calls made (visits that were not skipped) */
+  int64_t transfers;   /* transfers that changed a column */
+  int64_t pool_drops;  /* sections the pool could not serve */
+  double device_ms;    /* CUDA-event time around the call's kernels */
+} sm_relax_stats;
+int sm_relax(sm_context* ctx, int32_t max_passes, int32_t transferloop, sm_relax_stats* stats);
 
 /* WaterParticle::frequency/track, WindParticle::frequency (water.h:345-346, wind.h:48).
  * Any pointer may be NULL. */

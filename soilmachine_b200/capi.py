@@ -40,7 +40,7 @@ SYMBOLS = [
     "sm_lbm_step", "sm_lbm_get", "sm_lbm_advect", "sm_wind_use_lbm",
     "sm_create_group", "sm_group_size", "sm_group_rank", "sm_group_layout",
     "sm_snapshot_bytes", "sm_snapshot_save", "sm_snapshot_restore",
-    "sm_apply_layer",
+    "sm_apply_layer", "sm_relax",
 ]
 
 
@@ -88,6 +88,14 @@ class HydroBudget(C.Structure):
 class LayerStats(C.Structure):
     _fields_ = [("cells", C.c_int64), ("pushed", C.c_int64), ("free_slots", C.c_int64), ("emptied", C.c_int64),
                 ("device_ms", C.c_double)]
+
+    def asdict(self):
+        return {k: getattr(self, k) for k, _ in self._fields_}
+
+
+class RelaxStats(C.Structure):
+    _fields_ = [("passes", C.c_int64), ("stable", C.c_int64), ("visits", C.c_int64), ("transfers", C.c_int64),
+                ("pool_drops", C.c_int64), ("device_ms", C.c_double)]
 
     def asdict(self):
         return {k: getattr(self, k) for k, _ in self._fields_}
@@ -373,6 +381,16 @@ class Context:
             C.c_void_p(leftover.value if isinstance(leftover, C.c_void_p) else leftover)
         self._ck_strict(self.lib.sm_apply_layer(self.h, d, int(type), left, 1, int(bool(check)), C.byref(st)))
         return st, left
+
+    # ---- slope relaxation -------------------------------------------------------------------------------------------
+    def relax(self, max_passes, transferloop=0):
+        """sm_relax: up to max_passes passes of Particle::cascade(vec2(x, y), map, vp, transferloop) over every cell in
+        the phase order of the header; stops after the first pass that changes nothing.  Returns RelaxStats.  A refusal
+        (transferloop outside 0..3, max_passes < 1, a rank of a sharded map) raises with the map unchanged; sections the
+        pool could not serve warn, as the batches do, and are counted in pool_drops."""
+        st = RelaxStats()
+        self._ck(self.lib.sm_relax(self.h, int(max_passes), int(transferloop), C.byref(st)))
+        return st
 
     def set_soil_colors(self, rgba):
         rgba = np.ascontiguousarray(rgba, np.float32).reshape(-1, 4)

@@ -22,7 +22,9 @@
 #include "sm_lbm.cuh"
 #include "sm_snap.cuh"
 #include "sm_layer.cuh"
+#include "sm_relax.cuh"
 #include <cub/device/device_scan.cuh>
+#include <type_traits>
 
 #define KIND_WATER 0
 #define KIND_WIND 1
@@ -954,6 +956,40 @@ __global__ void __launch_bounds__(256) k_layer_apply(DevCtx c, const double* __r
     n += left > 0;
   }
   block_add_u64(n, emptied);
+}
+
+// ---- slope relaxation (sm_relax.cuh): one phase of a pass, one thread per phase cell of this context's strip ---------
+// Launch j of a call frees into ring[j & 1] and pops ring[(j & 1) ^ 1], which launch j - 1 filled and which nobody
+// appends to now.  The counts go to this rank's counter block; a launch that could not serve a section raises the stop
+// flag of every rank, and the launches after it return at once.
+template <bool MULTI>
+__global__ void __launch_bounds__(256) k_relax_phase(DevCtx c, int px, int py, int transferloop, unsigned int parity,
+                                                     const __grid_constant__ RelaxMaps m) {
+  __shared__ SoilDev s_soils[SM_MAX_SOILS];
+  __shared__ int stop;
+  for (int i = threadIdx.x; i < c.nsoils; i += blockDim.x) s_soils[i] = c.soils[i];
+  const int me = MULTI ? c.rank : 0;
+  if (threadIdx.x == 0) stop = (int)*((volatile unsigned long long*)&m.cnt[me][4]);
+  __syncthreads();
+  if (stop) return;
+  const int P = relax_period(transferloop);
+  const int x0 = MULTI ? c.rank * c.strip_w : 0, x1 = MULTI ? min(x0 + c.strip_w, c.dimx) : c.dimx;
+  const int fx = relax_first(x0, px, P);
+  const size_t nx = fx < x1 ? (size_t)((x1 - 1 - fx) / P + 1) : 0, ny = py < c.dimy ? (size_t)((c.dimy - 1 - py) / P + 1) : 0;
+  typename std::conditional<MULTI, RelaxMulti, RelaxDev>::type a(c, s_soils, parity, m, transferloop);
+  unsigned long long visits = 0;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < nx * ny; i += (size_t)gridDim.x * blockDim.x)
+    visits += relax_visit(a, fx + (int)(i / ny) * P, py + (int)(i % ny) * P, transferloop);
+  unsigned long long* const cnt = m.cnt[me];
+  block_add_u64(visits, &cnt[0]);
+  __syncthreads();
+  block_add_u64(a.rs.changes, &cnt[1]);
+  __syncthreads();
+  block_add_u64(a.rs.transfers, &cnt[2]);
+  if (a.rs.drops) {
+    atomicAdd(&cnt[3], a.rs.drops);
+    for (int q = 0; q < (MULTI ? c.nranks : 1); q++) m.cnt[q][4] = 1;
+  }
 }
 
 // Layermap::initialize, layermap.h:163-216: one thread per cell replays add() for every layer
@@ -3486,6 +3522,106 @@ int sm_apply_layer(sm_context* ctx, const double* delta, int32_t type, double* l
     add(in[(size_t)r].st);
   }
   if (stats) *stats = tot;
+  return SM_OK;
+}
+
+// ---- slope relaxation (sm_relax.cuh, DESIGN.md section 12) -------------------------------------------------------
+// One rank's share of a relax call: its stale bitmap and counter block, its timing events, and `ev`, recorded after
+// each of its phase launches, which every rank's next phase waits for.
+struct RelaxRank {
+  DevTmp t;
+  cudaEvent_t e0 = nullptr, e1 = nullptr, ev = nullptr;
+  unsigned long long cnt[SM_RELAX_CNT] = {};
+  ~RelaxRank() {
+    if (e0) cudaEventDestroy(e0);
+    if (e1) cudaEventDestroy(e1);
+    if (ev) cudaEventDestroy(ev);
+  }
+};
+
+int sm_relax(sm_context* ctx, int32_t max_passes, int32_t transferloop, sm_relax_stats* stats) {
+  if (transferloop < 0 || transferloop > 3 || max_passes < 1)
+    return fail(ctx, SM_ERR_INVALID, "sm_relax: range (transferloop 0..3, max_passes >= 1)");
+  if (!ctx->group && ctx->nranks > 1)
+    return fail(ctx, SM_ERR_INVALID, "sm_relax is not available on a rank of a sharded map (every phase needs every "
+                                     "rank's previous phase); a group (sm_create_group) offers it");
+  const int n = ctx->group ? ctx->group->n : 1;
+  sm_context* const* const R = ctx->group ? ctx->group->rank : &ctx;
+  if (R[0]->nsoils < 1) return fail(ctx, SM_ERR_INVALID, "soil table not set");
+  int rc;
+  if (ctx->group && (rc = grp_settle(ctx)) != SM_OK) return rc;
+  std::vector<RelaxRank> rk((size_t)n);
+  RelaxMaps m = {};
+  for (int r = 0; r < n; r++) {     // every cell stale, counters zero
+    sm_context* const c = R[r];
+    RelaxRank& k = rk[(size_t)r];
+    const size_t words = (c->lcells + 31) / 32;
+    if ((rc = snap_alloc(c, k.t, words * 4, (void**)&m.stale[r])) != SM_OK ||
+        (rc = snap_alloc(c, k.t, SM_RELAX_CNT * 8, (void**)&m.cnt[r])) != SM_OK)
+      return ctx->group ? grp_err(ctx, r, rc) : rc;
+    CK(cudaSetDevice(c->cfg.device));
+    CK(cudaMemsetAsync(m.stale[r], 0xFF, words * 4, c->stream));
+    CK(cudaMemsetAsync(m.cnt[r], 0, SM_RELAX_CNT * 8, c->stream));
+    CK(cudaEventCreate(&k.e0));
+    CK(cudaEventCreate(&k.e1));
+    CK(cudaEventCreateWithFlags(&k.ev, cudaEventDisableTiming));
+    CK(cudaEventRecord(k.e0, c->stream));
+  }
+  if (ctx->group) ctx->group->dirty = true;
+  const int P = relax_period(transferloop);
+  sm_relax_stats st = {};
+  unsigned long long changed = 0;
+  unsigned int j = 0;               // launch index of the call: its pool parity
+  for (int pass = 1; pass <= max_passes; pass++) {
+    for (int p = 0; p < P * P; p++, j++) {
+      // every rank's phase p - 1 is complete before any rank's phase p starts (only neighbours share columns, but the
+      // stop flag of a pool drop reaches every rank)
+      for (int r = 0; r < n; r++) {
+        sm_context* const c = R[r];
+        CK(cudaSetDevice(c->cfg.device));
+        if (n > 1 && j > 0)
+          for (int q = 0; q < n; q++) CK(cudaStreamWaitEvent(c->stream, rk[(size_t)q].ev, 0));
+        const size_t cells = (size_t)((c->x1 - c->x0 + P - 1) / P) * (size_t)((c->d.dimy + P - 1) / P);
+        const int blocks = (int)std::min<size_t>((cells + 255) / 256, (size_t)c->num_sms * 8);
+        if (n > 1) k_relax_phase<true><<<blocks, 256, 0, c->stream>>>(c->d, p / P, p % P, transferloop, j & 1u, m);
+        else k_relax_phase<false><<<blocks, 256, 0, c->stream>>>(c->d, p / P, p % P, transferloop, j & 1u, m);
+        c->launches++;
+        CK(cudaGetLastError());
+      }
+      if (n > 1)
+        for (int r = 0; r < n; r++) {
+          CK(cudaSetDevice(R[r]->cfg.device));
+          CK(cudaEventRecord(rk[(size_t)r].ev, R[r]->stream));
+        }
+    }
+    for (int r = 0; r < n; r++) {   // one counter block per rank and pass decides whether the call goes on
+      sm_context* const c = R[r];
+      CK(cudaSetDevice(c->cfg.device));
+      CK(cudaEventRecord(rk[(size_t)r].e1, c->stream));
+      CK(cudaMemcpyAsync(rk[(size_t)r].cnt, m.cnt[r], SM_RELAX_CNT * 8, cudaMemcpyDeviceToHost, c->stream));
+    }
+    unsigned long long tot[SM_RELAX_CNT] = {};
+    for (int r = 0; r < n; r++) {
+      CK(cudaSetDevice(R[r]->cfg.device));
+      CK(cudaStreamSynchronize(R[r]->stream));
+      for (int k = 0; k < SM_RELAX_CNT; k++) tot[k] += rk[(size_t)r].cnt[k];
+    }
+    st.passes = pass;
+    st.visits = (int64_t)tot[0];
+    st.transfers = (int64_t)tot[2];
+    st.pool_drops = (int64_t)tot[3];
+    st.stable = tot[1] == changed;
+    changed = tot[1];
+    if (st.pool_drops || st.stable) break;
+  }
+  if (ctx->group) ctx->group->dirty = false;    // every rank's stream was synchronised after the last pass
+  for (int r = 0; r < n; r++) {
+    float ms = 0.f;
+    CK(cudaEventElapsedTime(&ms, rk[(size_t)r].e0, rk[(size_t)r].e1));
+    st.device_ms = std::max(st.device_ms, (double)ms);
+  }
+  if (stats) *stats = st;
+  if (st.pool_drops) return fail(ctx, SM_ERR_POOL, "sm_relax: pool exhausted, sections dropped (the call stopped)");
   return SM_OK;
 }
 

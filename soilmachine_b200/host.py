@@ -109,6 +109,11 @@ class Simulation:
         typ = self.preset["soil_names"].index(soil) if isinstance(soil, str) else int(soil)
         return self.ctx.apply_layer(delta, typ, leftover=leftover)
 
+    def relax(self, max_passes, transferloop=0):
+        """Relax the slopes of the whole map (capi.Context.relax, sm_relax): Particle::cascade at every cell, pass after
+        pass in a fixed phase order, until a pass changes nothing or max_passes passes have run.  Returns the stats."""
+        return self.ctx.relax(max_passes, transferloop)
+
     def save(self, path):
         """Write the simulation to `path`: the snapshot of the map (columns and frequency arrays), the soil preset, the
         seed and the rand() draws made since srand.  A Simulation.load of the file continues the run with the same
