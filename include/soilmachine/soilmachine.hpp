@@ -18,6 +18,7 @@
 // Everything is header-only and written from scratch; vector types are minimal stand-ins that
 // convert implicitly from/to any type with .x/.y(/.z) members (so glm::ivec2 etc. can be passed).
 #pragma once
+#include <algorithm>
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
@@ -228,6 +229,23 @@ class Layermap {
     touch();
     ck(sm_relax(ctx, max_passes, transferloop, &st));
     return st;
+  }
+  // What lies under the surface, per cell, in one read-only call (sm_composition): for every type of `types`, the
+  // thickness of that soil inside the height window [lo, hi] (flags SM_COMP_BELOW_SURFACE: measured down from the
+  // surface; SM_COMP_PORE_WATER: the pore water it holds there).  Planar: out[i*dim.x*dim.y + x*dim.y + y].
+  std::vector<double> composition(const std::vector<SurfType>& types, double lo, double hi, int flags = 0) {
+    std::vector<int32_t> t(types.begin(), types.end());
+    std::vector<double> out(t.size() * (size_t)dim.x * (size_t)dim.y);
+    ck(sm_composition(ctx, t.data(), (int32_t)t.size(), lo, hi, flags, out.data(), 0, nullptr));
+    return out;
+  }
+  // The soil type at the heights z0 + k*dz, k < nz, of every cell of [lo.x, hi.x) x [lo.y, hi.y) (sm_voxelize): the
+  // first section met top -> bottom that contains the height, SM_VOXEL_NONE where none does.  Planar:
+  // out[k*W + (x - lo.x)*(hi.y - lo.y) + (y - lo.y)], W the window's cells.
+  std::vector<uint8_t> voxels(ivec2 lo, ivec2 hi, double z0, double dz, int nz) {
+    std::vector<uint8_t> out((size_t)std::max(nz, 0) * (size_t)std::max(hi.x - lo.x, 0) * (size_t)std::max(hi.y - lo.y, 0));
+    ck(sm_voxelize(ctx, lo.x, hi.x, lo.y, hi.y, z0, dz, nz, out.data(), 0, nullptr));
+    return out;
   }
 
   // ---- meshing (layermap.h:443-555) --------------------------------------------------------------------------

@@ -108,6 +108,8 @@ int sm_sync(sm_context* ctx);
  * calls that change the map return SM_ERR_INVALID on a sharded context; a group (sm_create_group) offers them.
  * sm_apply_layer works on a rank's own strip (same precondition).  sm_relax returns SM_ERR_INVALID on a sharded context:
  * each of its phases needs every rank's previous phase, a barrier across processes per phase; a group offers it.
+ * sm_composition and sm_voxelize read a rank's own strip (same precondition; a voxel window must lie inside the strip):
+ * each rank reads its own part and the caller joins the parts.
  * sm_peer_attach with use_ipc = 0 enables peer access to a blob's device when it differs from the context's. */
 #define SM_PEER_ARRAYS 23
 #define SM_PEER_SLOTS 24
@@ -153,6 +155,8 @@ int sm_hydro_issuer(sm_context* ctx, int32_t on);
  *   sm_launch_count: the ranks' launches summed; sm_last_error: the failing rank's message, prefixed "rank r: ";
  *   sm_mesh_device_ptr: SM_ERR_INVALID (there is no single device array: sm_group_rank + the rank's pointer);
  *   sm_peer_export, sm_peer_attach, sm_hydro_issuer: SM_ERR_INVALID (the group manages its ranks).
+ *   sm_composition, sm_voxelize: every rank computes its slice of the whole-map planes after every rank's work has
+ *     completed; device output lands in rank 0's buffer; the counts are summed, device_ms is the slowest rank's.
  * The group waits for every rank (sm_sync on each) before a call that reads or writes other ranks' strips, and only
  * when something was enqueued since the last wait.  SM_FLAG_BUDGET and SM_FLAG_CELL_BUDGET pass through to the ranks;
  * SM_FLAG_HYDRO_CELL_BUDGET with nranks > 1 is refused as by sm_create_sharded.  pool_capacity == 0 keeps the sharded
@@ -320,6 +324,63 @@ typedef struct sm_relax_stats {
   double device_ms;    /* CUDA-event time around the call's kernels */
 } sm_relax_stats;
 int sm_relax(sm_context* ctx, int32_t max_passes, int32_t transferloop, sm_relax_stats* stats);
+
+/* ---- strata views: what lies under the surface, per cell, in one call (DESIGN.md section 13) ------------------------
+ * Column terms are those of Sec32: the top record is top[cell], buried records are chained through `below`; "top ->
+ * bottom" is chain order.  H is the value sm_download_height returns for the cell: top.floor + top.size, or 0.0 for an
+ * empty column.  Both calls walk every section of the chain: a restored snapshot keeps `floor` verbatim (section 10), so
+ * floors need not be running sums and no walk stops early.  The accumulation order is fixed, so the results are
+ * deterministic and bit-identical on every sharding.
+ *
+ * sm_composition: types[0..ntypes) are distinct soil indices, 0 <= t < nsoils, 1 <= ntypes <= nsoils (type 0, Air, is
+ * the standing water).  The window lo <= hi: neither may be NaN, +-inf is allowed.  flags: SM_COMP_BELOW_SURFACE
+ * measures the window down from the surface; SM_COMP_PORE_WATER weights each overlap by the section's pore water.
+ * Per cell c:
+ *   [a, b] = BELOW_SURFACE ? [H - hi, H - lo] : [lo, hi]
+ *   out[i][c] = +0.0 for every slot i
+ *   for each section s of the column, top -> bottom:
+ *     ov = min(s.floor + s.size, b) - max(s.floor, a)
+ *     if ov > 0 and s.type == types[i]:
+ *       out[i][c] += PORE_WATER ? ov * s.saturation * (double)soils[s.type].porosity    // left to right
+ *                               : ov
+ * The output is planar: out[i * ncells + cell], cell order x*dimy + y, or (x - x0)*dimy + y on a rank's strip, so each
+ * slot is one raster and a rank's slice of a plane is contiguous.
+ *
+ * sm_voxelize: a window [x0, x1) x [y0, y1) in global coordinates, non-empty and inside the map (on a rank of a sharded
+ * map also inside the rank's strip); sample heights z_k = z0 + (double)k * dz for k < nz, z0 finite, dz > 0 finite,
+ * 1 <= nz <= SM_VOXEL_MAX_NZ (the library builds with -fmad=false: the expression means the same on host and device).
+ * With W the window's cells, out[k * W + (x - x0)*(y1 - y0) + (y - y0)] is the type of the FIRST section met walking
+ * top -> bottom with s.floor <= z_k < s.floor + s.size, or SM_VOXEL_NONE when no section contains z_k (above the column,
+ * under its bottom, an empty column).  Plane k is a horizontal slice at z_k; a window one cell wide is a vertical strata
+ * section.  "First met" decides only where sections overlap, which a restored snapshot can hold.
+ *
+ * Both calls are read-only: columns, pool, frequency arrays, budgets, per-cell maps, the mesh and an open batch are left
+ * exactly as they were.  on_device != 0: out is a device pointer on the context's device (rank 0's for a group);
+ * otherwise host memory, staged through at most 32 MB of device memory in cell-range chunks and copied into the planes
+ * with 2-D copies, so the extra device memory is bounded whatever the output size.  Every argument is checked before
+ * any launch; a refused call returns SM_ERR_INVALID with out untouched: a NaN bound, lo > hi, a type out of range or
+ * repeated, ntypes outside 1..nsoils, unknown flag bits, no soil table (sm_composition); an empty window or one outside
+ * the map or the rank's strip, z0 or dz not finite, dz <= 0, nz outside 1..SM_VOXEL_MAX_NZ (sm_voxelize); a null out.
+ * Rank of a sharded map: allowed on its own strip (its columns and buried sections live in its own pool, no peer
+ * access), with the precondition of the views above: every rank's earlier work has completed.  Group: the ranks are
+ * settled, each computes its slice; host output goes straight into the caller's whole-map planes, device output into
+ * rank 0's buffer (the kernel writes it where the rank shares rank 0's device, else through a rank-local staging buffer
+ * and a peer copy).  cells, sections and bytes_out are summed, device_ms is the slowest rank's; the result equals one
+ * context byte for byte.  stats may be NULL. */
+#define SM_COMP_BELOW_SURFACE 1
+#define SM_COMP_PORE_WATER 2
+#define SM_VOXEL_NONE 255
+#define SM_VOXEL_MAX_NZ 65536
+typedef struct sm_view_stats {
+  int64_t cells;       /* cells covered */
+  int64_t sections;    /* sections read */
+  int64_t bytes_out;   /* bytes written to out */
+  double device_ms;    /* CUDA-event time of the kernels */
+} sm_view_stats;
+int sm_composition(sm_context* ctx, const int32_t* types, int32_t ntypes, double lo, double hi, int32_t flags,
+                   double* out, int32_t on_device, sm_view_stats* stats);
+int sm_voxelize(sm_context* ctx, int32_t x0, int32_t x1, int32_t y0, int32_t y1, double z0, double dz, int32_t nz,
+                uint8_t* out, int32_t on_device, sm_view_stats* stats);
 
 /* WaterParticle::frequency/track, WindParticle::frequency (water.h:345-346, wind.h:48).
  * Any pointer may be NULL. */

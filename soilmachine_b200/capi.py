@@ -40,7 +40,7 @@ SYMBOLS = [
     "sm_lbm_step", "sm_lbm_get", "sm_lbm_advect", "sm_wind_use_lbm",
     "sm_create_group", "sm_group_size", "sm_group_rank", "sm_group_layout",
     "sm_snapshot_bytes", "sm_snapshot_save", "sm_snapshot_restore",
-    "sm_apply_layer", "sm_relax",
+    "sm_apply_layer", "sm_relax", "sm_composition", "sm_voxelize",
 ]
 
 
@@ -99,6 +99,19 @@ class RelaxStats(C.Structure):
 
     def asdict(self):
         return {k: getattr(self, k) for k, _ in self._fields_}
+
+
+class ViewStats(C.Structure):
+    _fields_ = [("cells", C.c_int64), ("sections", C.c_int64), ("bytes_out", C.c_int64), ("device_ms", C.c_double)]
+
+    def asdict(self):
+        return {k: getattr(self, k) for k, _ in self._fields_}
+
+
+SM_COMP_BELOW_SURFACE = 1
+SM_COMP_PORE_WATER = 2
+SM_VOXEL_NONE = 255
+SM_VOXEL_MAX_NZ = 65536
 
 
 CELL_TERMS = ("eroded", "deposited", "cascade_net")     # sm_last_cell_budget
@@ -391,6 +404,44 @@ class Context:
         st = RelaxStats()
         self._ck(self.lib.sm_relax(self.h, int(max_passes), int(transferloop), C.byref(st)))
         return st
+
+    # ---- strata views ------------------------------------------------------------------------------------------------
+    def composition(self, types, lo, hi, below_surface=False, pore_water=False, out=None):
+        """sm_composition: per cell, how much of each soil of `types` lies inside the height window [lo, hi] (measured
+        down from the surface with below_surface=True), or how much pore water it holds there (pore_water=True).
+        Returns a float64 array (len(types), x1 - x0, dimy) - the whole map, or this rank's strip of a sharded map.
+        out: a device pointer (device_alloc) of len(types) * (x1 - x0) * dimy doubles to write instead; then returns
+        None.  The call's ViewStats are kept in self.view_stats.  A refusal raises with nothing written."""
+        t = np.ascontiguousarray(np.atleast_1d(types), np.int32)
+        flags = (SM_COMP_BELOW_SURFACE if below_surface else 0) | (SM_COMP_PORE_WATER if pore_water else 0)
+        st = ViewStats()
+        res = None
+        if out is None:
+            res = np.empty((len(t), self.x1 - self.x0, self.dimy))
+            ptr, dev = res.ctypes.data_as(C.c_void_p), 0
+        else:
+            ptr, dev = C.c_void_p(out.value if isinstance(out, C.c_void_p) else out), 1
+        self._ck_strict(self.lib.sm_composition(self.h, _p(t, C.c_int32), len(t), C.c_double(lo), C.c_double(hi),
+                                                flags, ptr, dev, C.byref(st)))
+        self.view_stats = st
+        return res
+
+    def voxelize(self, x0, x1, y0, y1, z0, dz, nz, out=None):
+        """sm_voxelize: the soil type at the heights z0 + k*dz (k < nz) of every cell of the window [x0, x1) x [y0, y1)
+        (global coordinates; inside this rank's strip on a sharded map), the first section met top -> bottom that
+        contains the height, SM_VOXEL_NONE where none does.  Returns uint8 (nz, x1 - x0, y1 - y0); out: a device pointer
+        of that many bytes to write instead (returns None).  ViewStats in self.view_stats."""
+        st = ViewStats()
+        res = None
+        if out is None:
+            res = np.empty((max(int(nz), 0), max(x1 - x0, 0), max(y1 - y0, 0)), np.uint8)
+            ptr, dev = res.ctypes.data_as(C.c_void_p), 0
+        else:
+            ptr, dev = C.c_void_p(out.value if isinstance(out, C.c_void_p) else out), 1
+        self._ck_strict(self.lib.sm_voxelize(self.h, int(x0), int(x1), int(y0), int(y1), C.c_double(z0), C.c_double(dz),
+                                             int(nz), ptr, dev, C.byref(st)))
+        self.view_stats = st
+        return res
 
     def set_soil_colors(self, rgba):
         rgba = np.ascontiguousarray(rgba, np.float32).reshape(-1, 4)

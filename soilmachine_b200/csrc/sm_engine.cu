@@ -23,6 +23,7 @@
 #include "sm_snap.cuh"
 #include "sm_layer.cuh"
 #include "sm_relax.cuh"
+#include "sm_strata.cuh"
 #include <cub/device/device_scan.cuh>
 #include <type_traits>
 
@@ -956,6 +957,40 @@ __global__ void __launch_bounds__(256) k_layer_apply(DevCtx c, const double* __r
     n += left > 0;
   }
   block_add_u64(n, emptied);
+}
+
+// ---- strata views (sm_strata.cuh): one thread per cell, read-only --------------------------------------------------
+// the requested types: slot[t] = output slot of soil type t, -1 where t is not requested
+struct StrataSel { signed char slot[SM_MAX_SOILS]; };
+// cells [c0, c1) of this context's strip; slot i of cell i0 goes to out[i * stride + (i0 - c0)].  *nsec += sections read.
+__global__ void __launch_bounds__(256) k_strata_compose(DevCtx c, const __grid_constant__ StrataSel sel, int ntypes, double lo, double hi,
+                                                        int flags, size_t c0, size_t c1, double* __restrict__ out,
+                                                        size_t stride, unsigned long long* __restrict__ nsec) {
+  __shared__ float s_por[SM_MAX_SOILS];
+  __shared__ signed char s_slot[SM_MAX_SOILS];
+  for (int t = threadIdx.x; t < SM_MAX_SOILS; t += blockDim.x) {
+    s_por[t] = t < c.nsoils ? c.soils[t].porosity : 0.f;
+    s_slot[t] = sel.slot[t];
+  }
+  __syncthreads();
+  const StrataPool a{c.pool};
+  unsigned long long n = 0;
+  for (size_t i = c0 + (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < c1; i += (size_t)gridDim.x * blockDim.x)
+    n += strata_compose_cell(a, c.top[i], lo, hi, flags, s_slot, ntypes, s_por, out + (i - c0), stride);
+  block_add_u64(n, nsec);
+}
+// cells [j0, j1) of this context's part of a voxel window: part cell j is column xs + j / wy, row y0 + j % wy (global
+// coordinates; cx0 = the strip's first column); sample k of part cell j goes to out[k * stride + (j - j0)].
+__global__ void __launch_bounds__(256) k_strata_voxel(DevCtx c, int cx0, int xs, int y0, int wy, double z0, double dz,
+                                                      double rdz, uint32_t nz, size_t j0, size_t j1, unsigned char* __restrict__ out,
+                                                      size_t stride, unsigned long long* __restrict__ nsec) {
+  const StrataPool a{c.pool};
+  unsigned long long n = 0;
+  for (size_t j = j0 + (size_t)blockIdx.x * blockDim.x + threadIdx.x; j < j1; j += (size_t)gridDim.x * blockDim.x) {
+    const size_t x = (size_t)(xs - cx0) + j / (size_t)wy, y = (size_t)y0 + j % (size_t)wy;
+    n += strata_voxel_cell(a, c.top[x * c.dimy + y], z0, dz, rdz, nz, out + (j - j0), stride);
+  }
+  block_add_u64(n, nsec);
 }
 
 // ---- slope relaxation (sm_relax.cuh): one phase of a pass, one thread per phase cell of this context's strip ---------
@@ -3622,6 +3657,163 @@ int sm_relax(sm_context* ctx, int32_t max_passes, int32_t transferloop, sm_relax
   }
   if (stats) *stats = st;
   if (st.pool_drops) return fail(ctx, SM_ERR_POOL, "sm_relax: pool exhausted, sections dropped (the call stopped)");
+  return SM_OK;
+}
+
+}  // extern "C"
+
+// ---- strata views (sm_strata.cuh, DESIGN.md section 13) ----------------------------------------------------------
+namespace {
+struct StrataEvents {      // one kernel's timing events, destroyed with the call
+  int device = 0;
+  cudaEvent_t e0 = nullptr, e1 = nullptr;
+  StrataEvents() = default;
+  StrataEvents(const StrataEvents&) = delete;
+  StrataEvents& operator=(const StrataEvents&) = delete;
+  ~StrataEvents() {
+    if (!e0 && !e1) return;
+    cudaSetDevice(device);
+    if (e0) cudaEventDestroy(e0);
+    if (e1) cudaEventDestroy(e1);
+  }
+};
+}  // namespace
+
+// One context's part of a view: n cells, `planes` planes of esize-byte entries.  launch(lo, hi, out, stride, nsec)
+// enqueues the kernel that writes cells [lo, hi) of every plane to out[plane * stride + (cell - lo)].  dst: where cell 0
+// of plane 0 of this part goes, dpitch: the bytes from one plane to the next there.  direct: dst is on this context's
+// device and the kernel writes it in place; otherwise the planes go through a staging buffer of at most
+// SNAP_STAGE_BYTES, range by range, with 2-D copies to dst (host memory or another device).  Returns when dst is
+// written; st gets the sections read and the kernels' event time.
+template <class F>
+static int strata_part(sm_context* ctx, size_t n, size_t planes, size_t esize, unsigned char* dst, size_t dpitch,
+                       bool direct, F launch, sm_view_stats& st) {
+  CK(cudaSetDevice(ctx->cfg.device));
+  DevTmp t;
+  unsigned long long* d_n = nullptr;
+  int rc = snap_alloc(ctx, t, 8, (void**)&d_n);
+  if (rc != SM_OK) return rc;
+  CK(cudaMemsetAsync(d_n, 0, 8, ctx->stream));
+  const size_t chunk = direct ? std::max<size_t>(n, 1) : std::max<size_t>(1, SNAP_STAGE_BYTES / (planes * esize));
+  unsigned char* stage = nullptr;
+  if (!direct && (rc = snap_alloc(ctx, t, std::min(chunk, std::max<size_t>(n, 1)) * planes * esize, (void**)&stage)) != SM_OK)
+    return rc;
+  std::vector<StrataEvents> ev((n + chunk - 1) / chunk);
+  for (size_t lo = 0, j = 0; lo < n; lo += chunk, j++) {
+    const size_t hi = std::min(n, lo + chunk);
+    StrataEvents& e = ev[j];
+    e.device = ctx->cfg.device;
+    CK(cudaEventCreate(&e.e0));
+    CK(cudaEventCreate(&e.e1));
+    CK(cudaEventRecord(e.e0, ctx->stream));
+    launch(lo, hi, direct ? dst : stage, direct ? dpitch / esize : hi - lo, d_n);
+    ctx->launches++;
+    CK(cudaGetLastError());
+    CK(cudaEventRecord(e.e1, ctx->stream));
+    if (!direct) {      // the next range's kernel rewrites the staging buffer after this copy, in stream order
+      CK(cudaMemcpy2DAsync(dst + lo * esize, dpitch, stage, (hi - lo) * esize, (hi - lo) * esize, planes, cudaMemcpyDefault,
+                           ctx->stream));
+    }
+  }
+  unsigned long long nsec = 0;
+  CK(cudaMemcpyAsync(&nsec, d_n, 8, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  double ms = 0.0;
+  for (const StrataEvents& e : ev) {
+    float m = 0.f;
+    CK(cudaEventElapsedTime(&m, e.e0, e.e1));
+    ms += m;
+  }
+  st.cells += (int64_t)n;
+  st.sections += (int64_t)nsec;
+  st.bytes_out += (int64_t)(n * planes * esize);
+  st.device_ms = std::max(st.device_ms, ms);
+  return SM_OK;
+}
+
+// the ranks of ctx and whether rank r's kernels write device output in place (rank 0's device)
+static bool strata_direct(sm_context* ctx, sm_context* c, bool dev) {
+  return dev && (!ctx->group || c->cfg.device == ctx->group->rank[0]->cfg.device);
+}
+
+extern "C" {
+
+int sm_composition(sm_context* ctx, const int32_t* types, int32_t ntypes, double lo, double hi, int32_t flags,
+                   double* out, int32_t on_device, sm_view_stats* stats) {
+  const int n = ctx->group ? ctx->group->n : 1;
+  sm_context* const* const R = ctx->group ? ctx->group->rank : &ctx;
+  const int nsoils = R[0]->nsoils;
+  if (nsoils < 1) return fail(ctx, SM_ERR_INVALID, "soil table not set");
+  if (!types || !out) return fail(ctx, SM_ERR_INVALID, "sm_composition: null argument");
+  if (ntypes < 1 || ntypes > nsoils) return fail(ctx, SM_ERR_INVALID, "sm_composition: ntypes outside 1..nsoils");
+  if (std::isnan(lo) || std::isnan(hi) || lo > hi)
+    return fail(ctx, SM_ERR_INVALID, "sm_composition: the window needs lo <= hi, neither NaN");
+  if (flags & ~(SM_COMP_BELOW_SURFACE | SM_COMP_PORE_WATER)) return fail(ctx, SM_ERR_INVALID, "sm_composition: unknown flags");
+  StrataSel sel;
+  memset(sel.slot, -1, sizeof(sel.slot));
+  for (int i = 0; i < ntypes; i++) {
+    if (types[i] < 0 || types[i] >= nsoils) return fail(ctx, SM_ERR_INVALID, "sm_composition: type out of range");
+    if (sel.slot[types[i]] >= 0) return fail(ctx, SM_ERR_INVALID, "sm_composition: type repeated");
+    sel.slot[types[i]] = (signed char)i;
+  }
+  int rc;
+  if (ctx->group && (rc = grp_settle(ctx)) != SM_OK) return rc;
+  const bool dev = on_device != 0;
+  const size_t N = ctx->lcells;       // the cells of one plane: the whole map on a group, the strip on a rank
+  sm_view_stats st = {};
+  for (int r = 0; r < n; r++) {
+    sm_context* const c = R[r];
+    const size_t off = ctx->group ? (size_t)c->x0 * ctx->d.dimy : 0;
+    auto launch = [&](size_t a, size_t b, unsigned char* o, size_t stride, unsigned long long* d_n) {
+      k_strata_compose<<<c->num_sms * 8, 256, 0, c->stream>>>(c->d, sel, ntypes, lo, hi, flags, a, b, (double*)o, stride,
+                                                              d_n);
+    };
+    sm_view_stats part = {};
+    rc = strata_part(c, c->lcells, (size_t)ntypes, 8, (unsigned char*)(out + off), N * 8, strata_direct(ctx, c, dev),
+                     launch, part);
+    if (rc != SM_OK) return ctx->group ? grp_err(ctx, r, rc) : rc;
+    st.cells += part.cells; st.sections += part.sections; st.bytes_out += part.bytes_out;
+    st.device_ms = std::max(st.device_ms, part.device_ms);
+  }
+  if (ctx->group) ctx->group->dirty = false;     // every rank's stream was synchronised
+  if (stats) *stats = st;
+  return SM_OK;
+}
+
+int sm_voxelize(sm_context* ctx, int32_t x0, int32_t x1, int32_t y0, int32_t y1, double z0, double dz, int32_t nz,
+                uint8_t* out, int32_t on_device, sm_view_stats* stats) {
+  const int n = ctx->group ? ctx->group->n : 1;
+  sm_context* const* const R = ctx->group ? ctx->group->rank : &ctx;
+  if (!out) return fail(ctx, SM_ERR_INVALID, "sm_voxelize: null argument");
+  if (!(x0 < x1 && y0 < y1 && x0 >= ctx->x0 && x1 <= ctx->x1 && y0 >= 0 && y1 <= ctx->d.dimy))
+    return fail(ctx, SM_ERR_INVALID, "sm_voxelize: the window is empty or outside the map (or this rank's strip)");
+  if (!std::isfinite(z0) || !std::isfinite(dz) || !(dz > 0))
+    return fail(ctx, SM_ERR_INVALID, "sm_voxelize: z0 and dz must be finite, dz > 0");
+  if (nz < 1 || nz > SM_VOXEL_MAX_NZ) return fail(ctx, SM_ERR_INVALID, "sm_voxelize: nz outside 1..65536");
+  int rc;
+  if (ctx->group && (rc = grp_settle(ctx)) != SM_OK) return rc;
+  const bool dev = on_device != 0;
+  const double rdz = 1.0 / dz;      // the kernels estimate sample indices with it; the exact comparisons decide
+  const int wy = y1 - y0;
+  const size_t W = (size_t)(x1 - x0) * (size_t)wy;
+  sm_view_stats st = {};
+  for (int r = 0; r < n; r++) {
+    sm_context* const c = R[r];
+    const int xs = std::max(x0, c->x0), xe = std::min(x1, c->x1);
+    if (xs >= xe) continue;       // the window does not reach this rank's strip
+    auto launch = [&](size_t a, size_t b, unsigned char* o, size_t stride, unsigned long long* d_n) {
+      k_strata_voxel<<<c->num_sms * 8, 256, 0, c->stream>>>(c->d, c->x0, xs, y0, wy, z0, dz, rdz, (uint32_t)nz, a, b, o,
+                                                            stride, d_n);
+    };
+    sm_view_stats part = {};
+    rc = strata_part(c, (size_t)(xe - xs) * (size_t)wy, (size_t)nz, 1, out + (size_t)(xs - x0) * (size_t)wy, W,
+                     strata_direct(ctx, c, dev), launch, part);
+    if (rc != SM_OK) return ctx->group ? grp_err(ctx, r, rc) : rc;
+    st.cells += part.cells; st.sections += part.sections; st.bytes_out += part.bytes_out;
+    st.device_ms = std::max(st.device_ms, part.device_ms);
+  }
+  if (ctx->group) ctx->group->dirty = false;
+  if (stats) *stats = st;
   return SM_OK;
 }
 

@@ -109,6 +109,22 @@ class Simulation:
         typ = self.preset["soil_names"].index(soil) if isinstance(soil, str) else int(soil)
         return self.ctx.apply_layer(delta, typ, leftover=leftover)
 
+    def _soil(self, soil):
+        return self.preset["soil_names"].index(soil) if isinstance(soil, str) else int(soil)
+
+    def composition(self, soils, lo, hi, below_surface=False, pore_water=False):
+        """Per cell, how much of each soil (names of the preset's table or indices) lies inside the height window [lo,
+        hi], or how much pore water it holds there (capi.Context.composition, sm_composition): (len(soils), dimx, dimy)
+        float64."""
+        if isinstance(soils, (str, int, np.integer)):
+            soils = [soils]
+        return self.ctx.composition([self._soil(s) for s in soils], lo, hi, below_surface, pore_water)
+
+    def voxelize(self, x0, x1, y0, y1, z0, dz, nz):
+        """The soil index at the heights z0 + k*dz of every cell of [x0, x1) x [y0, y1) (capi.Context.voxelize,
+        sm_voxelize): (nz, x1 - x0, y1 - y0) uint8, 255 where no section holds the height."""
+        return self.ctx.voxelize(x0, x1, y0, y1, z0, dz, nz)
+
     def relax(self, max_passes, transferloop=0):
         """Relax the slopes of the whole map (capi.Context.relax, sm_relax): Particle::cascade at every cell, pass after
         pass in a fixed phase order, until a pass changes nothing or max_passes passes have run.  Returns the stats."""

@@ -70,6 +70,24 @@ def _layer_check(ctx, delta, type):
         return False, None, e
 
 
+def sum_view_stats(stats):
+    tot = capi.ViewStats()
+    for f, _ in capi.ViewStats._fields_:
+        vals = [getattr(s, f) for s in stats]
+        setattr(tot, f, max(vals) if f == "device_ms" else sum(vals))
+    return tot
+
+
+def voxel_part(ctx, x0, x1, y0, y1, z0, dz, nz):
+    """one rank's part of a voxel window: the window cut at the rank's strip (nz, 0, y1 - y0) when it misses the strip;
+    a window that is empty or leaves the map goes to the library whole, which refuses it"""
+    xs, xe = max(x0, ctx.x0), min(x1, ctx.x1)
+    if xs >= xe and 0 <= x0 < x1 <= ctx.dimx and 0 <= y0 < y1 <= ctx.dimy:
+        return np.empty((int(nz), 0, y1 - y0), np.uint8), None
+    out = ctx.voxelize(xs, xe, y0, y1, z0, dz, nz) if xs < xe else ctx.voxelize(x0, x1, y0, y1, z0, dz, nz)
+    return out, ctx.view_stats
+
+
 def sum_stats(stats):
     tot = capi.Stats()
     for f, _ in capi.Stats._fields_:
@@ -136,6 +154,22 @@ class VirtualShards:
         out = [c.apply_layer(delta[c.x0:c.x1], type, leftover=leftover) for c in self.ctx]
         self.sync()
         return sum_layer_stats([o[0] for o in out]), (np.concatenate([o[1] for o in out]) if leftover else None)
+
+    def composition(self, types, lo, hi, below_surface=False, pore_water=False):
+        """sm_composition over the whole map: every rank computes its strip, the strips are joined along x.  Returns
+        (len(types), dimx, dimy) float64; the summed ViewStats are kept in self.view_stats."""
+        self.sync()
+        parts = [c.composition(types, lo, hi, below_surface, pore_water) for c in self.ctx]
+        self.view_stats = sum_view_stats([c.view_stats for c in self.ctx])
+        return np.concatenate(parts, axis=1)
+
+    def voxelize(self, x0, x1, y0, y1, z0, dz, nz):
+        """sm_voxelize over the whole map: the window is cut at the strip edges, every rank voxelizes its part, the
+        parts are joined along x.  Returns (nz, x1 - x0, y1 - y0) uint8; summed ViewStats in self.view_stats."""
+        self.sync()
+        parts = [voxel_part(c, x0, x1, y0, y1, z0, dz, nz) for c in self.ctx]
+        self.view_stats = sum_view_stats([st for _, st in parts if st is not None])
+        return np.concatenate([p for p, _ in parts], axis=1)
 
     def heights(self):
         return np.concatenate([c.heights() for c in self.ctx], axis=0)
@@ -300,6 +334,18 @@ class DistShard:
         out = self.ctx.apply_layer(delta, type, leftover=leftover)
         self._settle()
         return out
+
+    def composition(self, types, lo, hi, below_surface=False, pore_water=False):
+        """sm_composition on this rank's strip: (len(types), x1 - x0, dimy) float64.  Every rank's earlier work must
+        have completed, so all ranks call it; the caller joins the strips along x."""
+        self._settle()
+        return self.ctx.composition(types, lo, hi, below_surface, pore_water)
+
+    def voxelize(self, x0, x1, y0, y1, z0, dz, nz):
+        """sm_voxelize on this rank's part of the window (global coordinates), the window cut at the strip edges:
+        (nz, part width, y1 - y0) uint8, of width 0 where the window misses the strip.  All ranks call it."""
+        self._settle()
+        return voxel_part(self.ctx, x0, x1, y0, y1, z0, dz, nz)[0]
 
     def run(self, kind, d_xy, n, max_sweeps=0):
         """launch this rank's sweep kernel (all ranks must call it), wait, return local stats"""
