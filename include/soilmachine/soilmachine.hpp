@@ -26,6 +26,7 @@
 #include <map>
 #include <stdexcept>
 #include <string>
+#include <utility>
 #include <vector>
 #include "../soilmachine_b200.h"
 #include "soilfile.hpp"
@@ -465,6 +466,19 @@ struct WaterParticle : Particle {
     map.ck(sm_water_flood(map.ctx, &st));
     detail::nested_ctor_draws(st.nested);
     return st;
+  }
+  // A batch whose particles flood at the end of the sweep they stop in (sm_water_run_flooding): later sweeps meet the
+  // batch's own ponds, closer to upstream's per-particle flood (SoilMachine.cpp:290-297) than run() + flood_batch().
+  template <class VP> static std::pair<sm_stats, sm_hydro_stats> run_flooding(Layermap& map, VP&, int NWATER) {
+    map.push_tables();
+    std::vector<float> xy = detail::spawn(map, NWATER);
+    sm_stats st{};
+    sm_hydro_stats hs{};
+    map.touch();
+    map.ck(sm_set_volume_factor(map.ctx, volumeFactor));
+    map.ck(sm_water_run_flooding(map.ctx, NWATER, xy.data(), 0, &st, &hs));
+    detail::nested_ctor_draws(hs.nested);
+    return {st, hs};
   }
   // WaterParticle::seep(map, vertexpool), water.h:335-343 / SoilMachine.cpp:300-301
   template <class VP> static sm_hydro_stats seep(Layermap& map, VP&) {

@@ -513,6 +513,23 @@ int sm_water_flood(sm_context* ctx, sm_hydro_stats* stats);
  * order, seep(cell) then the water-table cascade with spill 3.  Sharded map: as sm_water_flood (the issuing rank, the
  * whole map, warp executor). */
 int sm_seep(sm_context* ctx, sm_hydro_stats* stats);
+/* A water batch with sweep floods: the order of sm_water_run, except that after every sweep s the particles that
+ * stopped in it call flood() (water.h:123-145), in ascending index, before sweep s+1 starts; the live particles of
+ * sweep s+1 meet those ponds (Air tops, changed surfaces and heights).  Upstream floods each particle right after its
+ * own loop (SoilMachine.cpp:290-297); sm_water_run + sm_water_flood floods only once the whole batch has ended.  Each
+ * flood is atomic as in sm_water_flood and follows flood()'s own guard (volume >= minvol, spill left), so particles
+ * that left the map or evaporated do not flood; a particle floods at most once.  For n = 1 this equals sm_water_run +
+ * sm_water_flood.  max_sweeps > 0 stops after that many sweeps (and their floods); the survivors stay live, and
+ * sm_water_sweeps can resume them without floods.
+ * stats: the batch's counters (sweeps counts the sweeps that ran a particle; pool_drops covers the floods too).
+ * hstats: the floods' counters summed over the call (cells = 0).  device_ms of both = the whole call's device time.
+ * SM_FLAG_BUDGET: sm_last_budget covers the batch's particles, sm_last_hydro_budget every flood of the call, summed in
+ * execution order; SM_FLAG_CELL_BUDGET / SM_FLAG_HYDRO_CELL_BUDGET: the batch maps and the hydrology maps cover the
+ * same call.  The identity of the two budgets closes over the call: change of the whole map's height = the batch terms
+ * + the flood terms.  A group floods from rank 0 over the whole map, bit-identical to one context.  A rank of a map
+ * sharded over processes returns SM_ERR_INVALID (every sweep would need a flood issued across the processes). */
+int sm_water_run_flooding(sm_context* ctx, int32_t n, const float* spawn_xy, int32_t max_sweeps, sm_stats* stats,
+                          sm_hydro_stats* hstats);
 /* Mass budget of the last successful sm_water_flood or sm_seep call (contexts created with SM_FLAG_BUDGET; such a
  * context runs both on the warp executor whatever SM_HYDRO says).  Same rules as sm_budget: each term is a change
  * of column height (floor + top size) read right before and right after the column operation, accumulated in

@@ -41,6 +41,7 @@ SYMBOLS = [
     "sm_create_group", "sm_group_size", "sm_group_rank", "sm_group_layout",
     "sm_snapshot_bytes", "sm_snapshot_save", "sm_snapshot_restore",
     "sm_apply_layer", "sm_relax", "sm_composition", "sm_voxelize",
+    "sm_water_run_flooding",
 ]
 
 
@@ -498,6 +499,16 @@ class Context:
     def water_run(self, xy, max_sweeps=0):
         self._n["water"] = len(xy)
         return self._run(self.lib.sm_water_run, xy, max_sweeps)
+
+    def water_run_flooding(self, xy, max_sweeps=0):
+        """sm_water_run_flooding: a water batch whose particles flood at the end of the sweep they stop in, so later
+        sweeps of the batch meet the ponds.  Returns (Stats, HydroStats)."""
+        self._n["water"] = len(xy)
+        xy = np.ascontiguousarray(xy, np.float32)
+        st, hs = Stats(), HydroStats()
+        self._ck(self.lib.sm_water_run_flooding(self.h, len(xy), _p(xy, C.c_float), int(max_sweeps), C.byref(st),
+                                                C.byref(hs)))
+        return st, hs
 
     def wind_run(self, xy, max_sweeps=0):
         self._n["wind"] = len(xy)

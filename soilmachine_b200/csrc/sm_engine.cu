@@ -1489,22 +1489,29 @@ template <bool BUDGET, class S> __device__ __forceinline__ void hydro_totals_out
 // that ran its last step, and only there does `done` hold the dead marker: every rank clears done[0, n) before a
 // spawning launch (launch_run), and a rank writes a particle's `done` only while it holds the particle.  So the holder
 // is the one rank whose word is 0xFFFFFFFF; the flood reads the state there and leaves SM_DONE_FLOODED there.
-template <bool MULTI, bool BUDGET, bool CELLS = false>
-__global__ void __launch_bounds__(32) k_hydro_flood_w(DevCtx c, int n, HydroTotals* out, double* hcells,
-                                                      const __grid_constant__ FreqPeers fp) {
+// The flood phase over the particles [base0, n) by one warp.  RESUME: the counters and the budget sums continue from
+// what *out holds (k_hydro_flood_sweep, several flood phases in one call), else they start from zero.
+template <bool MULTI, bool BUDGET, bool CELLS, bool RESUME>
+__device__ __forceinline__ void hydro_flood_warp(const DevCtx& c, int base0, int n, HydroTotals* out, double* hcells,
+                                                 const FreqPeers& fp) {
   __shared__ SoilDev s_soils[SM_MAX_SOILS];
   __shared__ CoopScratch sc;
   __shared__ typename HydroScratchOf<BUDGET>::type hx;
   const int lane = threadIdx.x;
   for (int i = lane; i < c.nsoils; i += 32) s_soils[i] = c.soils[i];
-  hydro_budget_zero<BUDGET>(hx, lane);
+  if constexpr (RESUME && BUDGET) {
+    if (lane == 0) for (int k = 0; k < SM_HYDRO_BUDGET_SLOTS; k++) hx.bud[k] = out->bud[k];
+  } else {
+    hydro_budget_zero<BUDGET>(hx, lane);
+  }
   __syncwarp();
   WarpDev w{lane};
   ActiveMap none{};
   HydroBack<MULTI, BUDGET, CELLS> back(c, s_soils, none, false, hcells, &fp);
   CoopWin<HydroBack<MULTI, BUDGET, CELLS> > a(back, &sc);
   HydroCount hc{};
-  for (int base = 0; base < n; base += 32) {
+  if constexpr (RESUME) hc = out->hc;
+  for (int base = base0; base < n; base += 32) {
     const int i = base + lane;
     bool cand = false;
     int holder = 0;
@@ -1539,6 +1546,74 @@ __global__ void __launch_bounds__(32) k_hydro_flood_w(DevCtx c, int n, HydroTota
   }
   if (lane == 0) hydro_totals_out<BUDGET>(out, hc, hx);
 }
+template <bool MULTI, bool BUDGET, bool CELLS = false>
+__global__ void __launch_bounds__(32) k_hydro_flood_w(DevCtx c, int n, HydroTotals* out, double* hcells,
+                                                      const __grid_constant__ FreqPeers fp) {
+  hydro_flood_warp<MULTI, BUDGET, CELLS, false>(c, 0, n, out, hcells, fp);
+}
+
+// ---- sweep floods (sm_water_run_flooding): the batch advances one sweep per launch of k_sweep, and after each sweep
+// the particles that stopped in it flood, in ascending index, before the next sweep starts.
+// FloodGate: lives on the issuing context's device, zeroed by the host at the start of a call.
+//   hi1 / loinv  the flood candidates k_flood_gate found after the last sweep: indices [n - loinv, hi1), 0 = none
+//   ended        the batch had no live particle left after an earlier sweep
+//   sweeps       sweeps executed so far (a launch that finds no live particle executes none)
+struct FloodGate {
+  unsigned int hi1, loinv, ended, pad;
+  unsigned long long sweeps;
+};
+// After a sweep: count it, rotate the pool rings (below) and bound the particles that flood() will find (the predicate
+// of hydro_flood_warp: dead, volume >= minvol, not flooded yet), so that a sweep nobody stopped in costs no flood scan.
+// One pass over n words.
+template <bool MULTI>
+__global__ void __launch_bounds__(256) k_flood_gate(DevCtx c, int n, FloodGate* g) {
+  if (blockIdx.x == 0 && threadIdx.x == 0) {
+    if (!g->ended) g->sweeps++;
+    if (c.ctl->alive == 0) g->ended = 1u;     // MULTI: the issuing rank's copy holds the total over the ranks
+    // A one-sweep launch advances tag_base by 3, so without this every launch would free into the same ring and pop
+    // the same other ring, and the sweeps' frees would never be served again.  One unused tag more per sweep makes
+    // launch k free into ring[(t0 + k) % 3] and pop the ring launch k - 2 filled, as consecutive sweeps of one launch
+    // do.  Every rank's tags advance alike (the ranks' next launches wait for this kernel).
+    if constexpr (MULTI) {
+      for (int q = 0; q < c.nranks; q++) c.peer[q].ctl->tag_base += 1u;
+    } else {
+      c.ctl->tag_base += 1u;
+    }
+  }
+  const int stride = gridDim.x * blockDim.x;
+  for (int base = blockIdx.x * blockDim.x; base < n; base += stride) {     // warp-uniform trip count
+    const int i = base + (int)threadIdx.x;
+    bool cand = false;
+    if (i < n) {
+      if constexpr (MULTI) {
+        for (int q = 0; q < c.nranks; q++)
+          if (c.peer[q].done[i] == 0xFFFFFFFFu) {
+            cand = (c.peer[q].alive[i] == 0) && !(c.peer[q].pb[i].x < SM_MINVOL);
+            break;
+          }
+      } else {
+        cand = (c.alive[i] == 0) && !(c.pb[i].x < SM_MINVOL) && c.done[i] != SM_DONE_FLOODED;
+      }
+    }
+    const unsigned int m = __ballot_sync(0xFFFFFFFFu, cand);
+    if ((threadIdx.x & 31) == 0 && m) {
+      const int w0 = i;                                   // lane 0's index
+      atomicMax(&g->hi1, (unsigned int)(w0 + 32 - __clz((int)m)));
+      atomicMax(&g->loinv, (unsigned int)(n - (w0 + __ffs((int)m) - 1)));
+    }
+  }
+}
+// The flood phase after one sweep: hydro_flood_warp over the gate's range, counters and budget continuing from *out
+// (zeroed by the host at the start of the call); then the gate is cleared for the next sweep.
+template <bool MULTI, bool BUDGET, bool CELLS = false>
+__global__ void __launch_bounds__(32) k_hydro_flood_sweep(DevCtx c, int n, HydroTotals* out, double* hcells,
+                                                          const __grid_constant__ FreqPeers fp, FloodGate* g) {
+  const unsigned int hi1 = g->hi1, loinv = g->loinv;
+  if (hi1 == 0u) return;
+  hydro_flood_warp<MULTI, BUDGET, CELLS, true>(c, (n - (int)loinv) & ~31, (int)hi1, out, hcells, fp);
+  if (threadIdx.x == 0) { g->hi1 = 0u; g->loinv = 0u; }
+}
+
 template <bool MULTI, bool BUDGET, bool CELLS = false>
 __global__ void __launch_bounds__(32) k_hydro_seep_w(DevCtx c, ActiveMap am, HydroTotals* out, double* hcells,
                                                      const __grid_constant__ FreqPeers fp) {
@@ -1591,6 +1666,7 @@ struct sm_context {
   unsigned long long* d_act = nullptr;   // active-cell index of the seep pass (allocated on first use)
   unsigned long long act_words = 0;
   HydroTotals* d_hydro = nullptr;
+  FloodGate* d_gate = nullptr;    // sm_water_run_flooding (allocated on first use)
   double hydro_bud[SM_HYDRO_BUDGET_SLOTS] = {};   // budget of the last successful hydrology call (SM_FLAG_BUDGET)
   bool hydro_bud_valid = false;
   // per-cell budget maps (SM_FLAG_CELL_BUDGET): 3 f64 per cell of the strip, interleaved; every rank's, by rank
@@ -1653,7 +1729,7 @@ void sm_destroy(sm_context* ctx) {
   for (int i = 0; i < 3; i++) cudaFree(d.lmask[i]);
   for (int i = 0; i < 2; i++) { cudaFree(d.head[i]); cudaFree(d.node[i]); }
   cudaFree(ctx->d_verts); cudaFree(ctx->d_colors); cudaFree(d.dbg);
-  cudaFree(ctx->d_act); cudaFree(ctx->d_hydro); cudaFree(ctx->d_cells); cudaFree(ctx->d_hcells);
+  cudaFree(ctx->d_act); cudaFree(ctx->d_hydro); cudaFree(ctx->d_gate); cudaFree(ctx->d_cells); cudaFree(ctx->d_hcells);
   cudaFree(ctx->lbm.F[0]); cudaFree(ctx->lbm.F[1]); cudaFree(ctx->lbm.B); cudaFree(ctx->lbm.RHO); cudaFree(ctx->lbm.V);
   cudaFree(ctx->d_spawn); cudaFree(ctx->d_scratch); cudaFree(ctx->d_iscratch); cudaFree(ctx->d_cellres);
   if (ctx->h_ctl) cudaFreeHost(ctx->h_ctl);
@@ -2719,6 +2795,118 @@ int sm_last_hydro_cell_budget(sm_context* ctx, double* eroded, double* deposited
       if (out[k]) for (size_t i = 0; i < n; i++) out[k][c0 + i] = m[i * SM_HYDRO_CELL_TERMS + k];
   }
   return SM_OK;
+}
+
+// ---- sweep floods: a water batch whose particles flood at the end of the sweep they stop in -------------------------
+// Every sweep is one launch of the sweep kernel (max_sweeps = 1; the first spawns, the others resume), followed on the
+// issuing context's stream by k_flood_gate and k_hydro_flood_sweep.  Segments are enqueued in rounds; the live count
+// is read back once per round, so the host waits once per round, not once per sweep.  A launch after the batch has
+// ended finds no live particle and no candidate and returns at once.  DESIGN.md K6 "Sweep floods".
+static int flood_phase(sm_context* ctx, int n) {
+  const int blocks = (int)std::max<long long>(1, std::min<long long>(((long long)n + 255) / 256, (long long)ctx->num_sms * 4));
+  const FreqPeers& fp = ctx->freq_of;
+  if (ctx->nranks > 1) {
+    k_flood_gate<true><<<blocks, 256, 0, ctx->stream>>>(ctx->d, n, ctx->d_gate);
+    if (ctx->d.bud) k_hydro_flood_sweep<true, true><<<1, 32, 0, ctx->stream>>>(ctx->d, n, ctx->d_hydro, nullptr, fp, ctx->d_gate);
+    else k_hydro_flood_sweep<true, false><<<1, 32, 0, ctx->stream>>>(ctx->d, n, ctx->d_hydro, nullptr, fp, ctx->d_gate);
+  } else {
+    k_flood_gate<false><<<blocks, 256, 0, ctx->stream>>>(ctx->d, n, ctx->d_gate);
+    if (ctx->d_hcells)
+      k_hydro_flood_sweep<false, true, true><<<1, 32, 0, ctx->stream>>>(ctx->d, n, ctx->d_hydro, ctx->d_hcells, fp, ctx->d_gate);
+    else if (ctx->d.bud) k_hydro_flood_sweep<false, true><<<1, 32, 0, ctx->stream>>>(ctx->d, n, ctx->d_hydro, nullptr, fp, ctx->d_gate);
+    else k_hydro_flood_sweep<false, false><<<1, 32, 0, ctx->stream>>>(ctx->d, n, ctx->d_hydro, nullptr, fp, ctx->d_gate);
+  }
+  ctx->launches += 2;
+  CK(cudaGetLastError());
+  return SM_OK;
+}
+// one sweep of the batch and the floods of the particles that stopped in it
+static int flood_segment(sm_context* ctx, int n, const float* h_xy, bool first) {
+  if (!ctx->group) {
+    const int rc = launch_run(ctx, KIND_WATER, n, first ? ctx->d_spawn : nullptr, 1);
+    return rc != SM_OK ? rc : flood_phase(ctx, n);
+  }
+  sm_group& G = *ctx->group;
+  sm_context* const c0 = G.rank[0];
+  int rc = first ? grp_run(ctx, KIND_WATER, n, h_xy, nullptr, 1, true)
+                 : grp_each(ctx, [&](sm_context* c, int) { return launch_run(c, KIND_WATER, c->cur_n, nullptr, 1); });
+  if (rc != SM_OK) return rc;
+  // the flood reads and writes every strip: rank 0 waits for every rank's sweep, every rank's next sweep for the flood
+  for (int r = 1; r < G.n; r++) {
+    sm_context* const c = G.rank[r];
+    CK(cudaSetDevice(c->cfg.device));
+    CK(cudaEventRecord(c->evt0, c->stream));
+    CK(cudaSetDevice(c0->cfg.device));
+    CK(cudaStreamWaitEvent(c0->stream, c->evt0, 0));
+  }
+  rc = flood_phase(c0, n);
+  if (rc != SM_OK) return grp_err(ctx, 0, rc);
+  CK(cudaEventRecord(G.ev, c0->stream));
+  for (int r = 1; r < G.n; r++) {
+    sm_context* const c = G.rank[r];
+    CK(cudaSetDevice(c->cfg.device));
+    CK(cudaStreamWaitEvent(c->stream, G.ev, 0));
+  }
+  return SM_OK;
+}
+int sm_water_run_flooding(sm_context* ctx, int32_t n, const float* xy, int32_t max_sweeps, sm_stats* st,
+                          sm_hydro_stats* hst) {
+  if (!ctx->group && ctx->nranks > 1)
+    return fail(ctx, SM_ERR_INVALID, "sm_water_run_flooding: not available on a rank of a sharded map (use a group)");
+  if (n < 0 || n > ctx->max_particles) return fail(ctx, SM_ERR_INVALID, "batch larger than max_particles");
+  if (n > 0 && !xy) return fail(ctx, SM_ERR_INVALID, "null spawn list");
+  sm_context* const c0 = ctx->group ? ctx->group->rank[0] : ctx;
+  int rc = hydro_ready(c0);
+  if (rc != SM_OK) return ctx->group ? grp_err(ctx, 0, rc) : rc;
+  if (!c0->d_gate) CK(cudaMalloc(&c0->d_gate, sizeof(FloodGate)));
+  CK(cudaEventRecord(c0->evt0, c0->stream));
+  rc = hydro_cells_reset(c0);
+  if (rc != SM_OK) return rc;
+  CK(cudaMemsetAsync(c0->d_gate, 0, sizeof(FloodGate), c0->stream));
+  if (n == 0) CK(cudaMemsetAsync(&c0->d_gate->ended, 1, 1, c0->stream));
+  CK(cudaMemsetAsync(c0->d_hydro, 0, sizeof(HydroTotals), c0->stream));
+  if (!ctx->group) {
+    if (n) CK(cudaMemcpyAsync(ctx->d_spawn, xy, (size_t)n * 8, cudaMemcpyHostToDevice, ctx->stream));
+    rc = zero_counters(ctx);
+    if (rc == SM_OK) rc = new_batch(ctx, KIND_WATER, n);
+    if (rc != SM_OK) return rc;
+  }
+  long long done = 0;
+  for (int round = 16;; round = std::min(2 * round, 256)) {
+    const long long k = max_sweeps > 0 ? std::min<long long>(round, (long long)max_sweeps - done) : round;
+    for (long long j = 0; j < k; j++) {
+      rc = flood_segment(ctx, n, xy, done + j == 0);
+      if (rc != SM_OK) return rc;
+    }
+    done += k;
+    if (max_sweeps > 0 && done >= max_sweeps) break;
+    CK(cudaSetDevice(c0->cfg.device));
+    CK(cudaMemcpyAsync(&c0->h_ctl->alive, &c0->d.ctl->alive, sizeof(unsigned long long), cudaMemcpyDeviceToHost,
+                             c0->stream));
+    CK(cudaStreamSynchronize(c0->stream));
+    if (c0->h_ctl->alive == 0) break;
+  }
+  // the batch's sweep count replaces what the last launch counted (sm_last_stats reads it from the issuer's counters)
+  CK(cudaSetDevice(c0->cfg.device));
+  CK(cudaMemcpyAsync(&c0->d.ctl->sweeps, &c0->d_gate->sweeps, sizeof(unsigned long long), cudaMemcpyDeviceToDevice,
+                           c0->stream));
+  CK(cudaEventRecord(c0->evt1, c0->stream));
+  sm_stats s;
+  memset(&s, 0, sizeof(s));
+  rc = ctx->group ? grp_last_stats(ctx, &s) : sm_last_stats(ctx, &s);
+  sm_hydro_stats h;
+  memset(&h, 0, sizeof(h));
+  const int hrc = hydro_finish(c0, &h);
+  float ms = 0.f;
+  CK(cudaEventElapsedTime(&ms, c0->evt0, c0->evt1));
+  s.device_ms = ms;
+  h.device_ms = ms;
+  h.classify_ms = 0.0;
+  if (st) *st = s;
+  if (hst) *hst = h;
+  if (ctx->group) for (int r = 0; r < ctx->group->n; r++) ctx->group->rank[r]->mesh_valid = false;
+  if (rc != SM_OK) return rc;
+  return hrc != SM_OK && ctx->group ? grp_err(ctx, 0, hrc) : hrc;
 }
 
 // stepping interface: *_begin runs the prologue only (spawn + bins), *_sweeps(k) resumes the batch

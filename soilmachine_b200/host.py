@@ -75,26 +75,37 @@ class Simulation:
         self.ctx.set_soil_colors(self.preset["colors"])
         self.ctx.initialize(self.seed, self.preset["layers"])   # Layermap(SEED, dim), SoilMachine.cpp:83
 
-    def frame(self, nwater, nwind, water_xy=None, wind_xy=None, hydrology=False, water_chunk=0):
+    def frame(self, nwater, nwind, water_xy=None, wind_xy=None, hydrology=False, water_chunk=0, floods="batch"):
         """SoilMachine.cpp:287-320.  hydrology=False: the hot path only (flood disabled, no seep pass);
         True: the water batch is followed by its floods and by the seep pass (self.last_hydrology holds the
         counter sets).  water_chunk > 0 splits the frame's water particles into lockstep batches of that
         size, each followed by its floods: upstream floods every particle right after its own loop, so later
         particles of a frame meet the ponds earlier ones left; smaller chunks follow that interleaving more
         closely (chunk 1 = upstream's order) at the price of fewer particles in flight (DESIGN.md K6).
+        floods="sweep" (with hydrology=True): each water batch floods its particles at the end of the sweep they stop
+        in (capi.Context.water_run_flooding), so the batch's later sweeps meet its own ponds; "batch" (the default)
+        floods them once the batch has ended.
         Returns (water_stats of the last batch, wind_stats)."""
+        if floods not in ("batch", "sweep"):
+            raise ValueError("floods must be 'batch' or 'sweep'")
+        if floods == "sweep" and not hydrology:
+            raise ValueError("floods='sweep' needs hydrology=True")
         ws = ds = None
         self.last_hydrology = None
         if nwater:
             xy = water_xy if water_xy is not None else spawn_list(nwater, self.dimx, self.dimy)
             chunk = int(water_chunk) if (hydrology and water_chunk and water_chunk > 0) else len(xy)
-            floods = []
+            flooded = []
             for i in range(0, len(xy), chunk):
+                if floods == "sweep":
+                    ws, fs = self.ctx.water_run_flooding(xy[i:i + chunk])
+                    flooded.append(fs)
+                    continue
                 ws = self.ctx.water_run(xy[i:i + chunk])
                 if hydrology:
-                    floods.append(self.ctx.water_flood())
+                    flooded.append(self.ctx.water_flood())
             if hydrology:
-                self.last_hydrology = (floods, self.ctx.seep())
+                self.last_hydrology = (flooded, self.ctx.seep())
         if nwind:
             xy = wind_xy if wind_xy is not None else spawn_list(nwind, self.dimx, self.dimy)
             ds = self.ctx.wind_run(xy)
