@@ -70,6 +70,9 @@ struct PeerPtrs {
   double* bud;
   unsigned int* fin;
   unsigned int* lmask[3];
+#ifdef SM_AUDIT_HANDOFF
+  unsigned int* relz;
+#endif
 };
 
 struct DevCtx {
@@ -105,6 +108,9 @@ struct DevCtx {
   int nranks, rank, strip_w;
   unsigned long long* dbg;       // -DSM_PROFILE: per-sweep (clock64, live particles) of the last launch
   PeerPtrs peer[SM_MAX_RANKS];
+#ifdef SM_AUDIT_HANDOFF
+  unsigned int* relz;            // audit builds: tag of the last sweep whose hand-off this particle released
+#endif
 };
 
 template <bool MULTI> __device__ __forceinline__ int owner_of_x(const DevCtx& c, int x) {

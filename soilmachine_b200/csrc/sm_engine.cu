@@ -1726,6 +1726,9 @@ void sm_destroy(sm_context* ctx) {
   cudaFree(d.top); cudaFree(d.pool); cudaFree(d.ringbuf[0]); cudaFree(d.ringbuf[1]); cudaFree(d.ringbuf[2]);
   cudaFree(d.wfreq); cudaFree(d.wtrack); cudaFree(d.windfreq); cudaFree(ctx->d_soils);
   cudaFree(d.ctl); cudaFree(d.pa); cudaFree(d.pb); cudaFree(d.pc); cudaFree(d.alive); cudaFree(d.done); cudaFree(d.fin); cudaFree(d.mv); cudaFree(d.bud);
+#ifdef SM_AUDIT_HANDOFF
+  cudaFree(d.relz);
+#endif
   for (int i = 0; i < 3; i++) cudaFree(d.lmask[i]);
   for (int i = 0; i < 2; i++) { cudaFree(d.head[i]); cudaFree(d.node[i]); }
   cudaFree(ctx->d_verts); cudaFree(ctx->d_colors); cudaFree(d.dbg);
@@ -1819,6 +1822,9 @@ static int create_impl(const sm_config* cfg, int nranks, int rank, int share, sm
     CK(cudaMalloc(&d.pa, N * sizeof(float4))); CK(cudaMalloc(&d.pb, N * sizeof(double2)));
     CK(cudaMalloc(&d.pc, N * sizeof(uint2))); CK(cudaMalloc(&d.alive, N)); CK(cudaMalloc(&d.done, N * 4));
     CK(cudaMalloc(&d.fin, N * 4)); CK(cudaMalloc(&d.mv, N * 8));
+#ifdef SM_AUDIT_HANDOFF
+    CK(cudaMalloc(&d.relz, N * 4)); CK(cudaMemsetAsync(d.relz, 0, N * 4, ctx->stream));
+#endif
     for (int i = 0; i < 3; i++) {
       CK(cudaMalloc(&d.lmask[i], (N / 32 + 2) * sizeof(unsigned int)));
       CK(cudaMemsetAsync(d.lmask[i], 0, (N / 32 + 2) * sizeof(unsigned int), ctx->stream));
@@ -1920,6 +1926,12 @@ int sm_shard_range(sm_context* ctx, int32_t* x0, int32_t* x1) {
 }
 
 // ---- peers of a sharded map ----------------------------------------------------------------------------
+// audit builds (-DSM_AUDIT_HANDOFF) exchange one more array, the hand-off records (relz)
+#ifdef SM_AUDIT_HANDOFF
+#define SM_PEER_USED (SM_PEER_ARRAYS + 1)
+#else
+#define SM_PEER_USED SM_PEER_ARRAYS
+#endif
 static void own_ptrs(sm_context* ctx, void** p) {
   DevCtx& d = ctx->d;
   p[0] = d.top; p[1] = d.pool; p[2] = d.ringbuf[0]; p[3] = d.ringbuf[1]; p[4] = d.ctl; p[5] = d.pa; p[6] = d.pb;
@@ -1927,6 +1939,9 @@ static void own_ptrs(sm_context* ctx, void** p) {
   p[14] = d.ringbuf[2]; p[15] = d.bud; p[16] = d.fin; p[17] = d.lmask[0]; p[18] = d.lmask[1]; p[19] = d.lmask[2];
   p[20] = ctx->d_cells;
   p[21] = d.wfreq; p[22] = d.wtrack;    // each its own cudaMalloc (create_impl), as cudaIpcGetMemHandle needs
+#ifdef SM_AUDIT_HANDOFF
+  p[SM_PEER_ARRAYS] = d.relz;
+#endif
 }
 static void fill_peer(PeerPtrs& P, void* const* p, unsigned long long pool_cap) {
   P.top = (Sec32*)p[0]; P.pool = (Sec32*)p[1]; P.ringbuf[0] = (uint32_t*)p[2]; P.ringbuf[1] = (uint32_t*)p[3];
@@ -1936,6 +1951,9 @@ static void fill_peer(PeerPtrs& P, void* const* p, unsigned long long pool_cap) 
   P.ringbuf[2] = (uint32_t*)p[14]; P.bud = (double*)p[15]; P.fin = (unsigned int*)p[16];
   P.lmask[0] = (unsigned int*)p[17]; P.lmask[1] = (unsigned int*)p[18]; P.lmask[2] = (unsigned int*)p[19];
   P.pool_cap = pool_cap;
+#ifdef SM_AUDIT_HANDOFF
+  P.relz = (unsigned int*)p[SM_PEER_ARRAYS];
+#endif
 }
 int sm_peer_export(sm_context* ctx, sm_peer_blob* out) {
   if (ctx->group) return fail(ctx, SM_ERR_INVALID, "a group manages its ranks' peers itself (sm_group_rank gives the rank contexts)");
@@ -1944,7 +1962,7 @@ int sm_peer_export(sm_context* ctx, sm_peer_blob* out) {
   memset(out, 0, sizeof(*out));
   void* p[SM_PEER_SLOTS] = {};
   own_ptrs(ctx, p);
-  for (int i = 0; i < SM_PEER_ARRAYS; i++) {
+  for (int i = 0; i < SM_PEER_USED; i++) {
     out->ptr[i] = (uint64_t)(uintptr_t)p[i];
     if (!p[i]) continue;                      // optional array (mass budget, per-cell maps) not allocated
     cudaIpcMemHandle_t h;
@@ -1985,9 +2003,9 @@ int sm_peer_attach(sm_context* ctx, const sm_peer_blob* blobs, int32_t nblobs, i
     if (q == ctx->rank) {
       own_ptrs(ctx, p);
     } else if (!use_ipc) {
-      for (int i = 0; i < SM_PEER_ARRAYS; i++) p[i] = (void*)(uintptr_t)b.ptr[i];   // same process
+      for (int i = 0; i < SM_PEER_USED; i++) p[i] = (void*)(uintptr_t)b.ptr[i];   // same process
     } else {
-      for (int i = 0; i < SM_PEER_ARRAYS; i++) {
+      for (int i = 0; i < SM_PEER_USED; i++) {
         if (!b.ptr[i]) continue;
         cudaIpcMemHandle_t h;
         memcpy(&h, b.ipc[i], 64);
@@ -2528,6 +2546,7 @@ int sm_last_stats(sm_context* ctx, sm_stats* st) {
     st->pool_drops = (int64_t)h.drops; st->alive = (int64_t)h.alive; st->device_ms = ms;
   }
   if (h.err & (1u << 4)) return fail(ctx, SM_ERR_REACH, "a particle step left its conflict box");
+  if (h.err & (1u << 6)) return fail(ctx, SM_ERR_REACH, "a waiter acquired a hand-off that was not released (audit build)");
   if (h.err & (1u << 3)) return fail(ctx, SM_ERR_POOL, "section pool exhausted (sections were dropped)");
   return SM_OK;
 }

@@ -13,6 +13,7 @@
 // Included by sm_engine.cu after the bin / particle-I/O helpers.
 #pragma once
 #include "sm_coop.cuh"
+#include "sm_handoff.cuh"
 
 // Block shape by kind: warps (= particles in flight) per block and resident blocks per SM the kernel is compiled for
 // (which sets the register cap).  Wind: 2 x 10 warps, a 96-register cap (65536 / 640 threads) that halves the spills
@@ -146,12 +147,13 @@ template <bool MULTI, bool BUDGET = false, bool CELLS = false> struct DevBack : 
 struct __align__(32) WarpSmem {
   CoopScratch cs;
   uint32_t blk[SM_SW_NEARX];   // in-range lower-index particles of this sweep (rank in bits 28-31 on a sharded map)
-  uint32_t pred[12];     // per-bin predecessors (largest lower index in each of the 3x3 bins)
+  uint32_t pred[12];     // per-bin predecessors (largest lower index in each of the 3x3 bins); wind: in-range lower-index count per bin
   uint32_t cnt;
   uint32_t m0[SM_SW_NEARX / 32];   // exact schedule: bit l = entry l can delay move() (its box can meet plus(ipos))
   uint32_t n1[SM_SW_NEARX / 32];   // exact schedule: bit l = entry l still unresolved after the wait to move
   uint32_t remote;       // exact schedule: some in-range lower-index particle is executed by another rank
-  uint32_t succ;         // a higher-index particle lives in the 3x3 bins: somebody may wait for this particle's hand-off
+  uint32_t succ;         // somebody may wait for this particle's hand-off: a higher-index particle lives in the 3x3 bins
+                         // (wind: one in range, sm_handoff.cuh)
   uint32_t blkxy[SM_SW_NEARX];   // exact schedule: packed (ipos, reach) of entry l, as in the bin node
 };
 
@@ -163,7 +165,8 @@ __device__ __forceinline__ float next_dy(const WindP& p) { return p.sz; }
 template <class W, class A> __device__ __forceinline__ int do_step_coop(W& w, A& a, WaterP& p) { return water_step_coop(w, a, p); }
 template <class W, class A> __device__ __forceinline__ int do_step_coop(W& w, A& a, WindP& p) { return wind_step_coop(w, a, p); }
 
-// Conflict detection for one particle and one sweep, nine lanes = the 3x3 bins around ipos.  Two steps are
+// Conflict detection for one water particle (and, on a sharded map, a wind particle) and one sweep, nine lanes = the
+// 3x3 bins around ipos; wind on one rank: wind_scan.  Two steps are
 // ordered iff their published boxes can meet (|dipos|_inf <= R_A + R_B).  Sparse case: every lower-index
 // particle in range gets a polling lane, plus the own-bin predecessor.  Crowded case (more than SM_SW_NEAR in
 // range): the nine per-bin predecessors.  Every particle always waits for its own-bin predecessor, hence
@@ -228,6 +231,23 @@ __device__ __forceinline__ uint32_t coop_scan(const DevCtx& c, WarpSmem& ws, int
   return lane < 9 ? ws.pred[lane] : SM_NIL;
 }
 
+#ifdef SM_AUDIT_HANDOFF
+// Audit builds (-DSM_AUDIT_HANDOFF, not the product): a particle that publishes its hand-off with a release first
+// records the sweep in relz[pid]; a waiter that has acquired the hand-off of `tgt` checks that it was a release of this
+// sweep, and counts the miss (error bit 6, dbg row 16381) instead of racing on silently.
+template <bool MULTI>
+__device__ __forceinline__ void audit_acquired(const DevCtx& c, uint32_t tgt, unsigned int tag) {
+  const unsigned int* rz = MULTI ? c.peer[tgt >> 28].relz : c.relz;
+  if (ld_relaxed_u32(&rz[tgt & 0x0FFFFFFFu]) != tag) {
+    atomicOr(&c.ctl->err, 1u << 6);
+    atomicAdd(&c.dbg[8 * 16381], 1ull);
+  }
+}
+#define SM_AUDIT_RELEASED(c, pid, tag) ((c).relz[pid] = (tag))
+#else
+#define SM_AUDIT_RELEASED(c, pid, tag) ((void)0)
+#endif
+
 // spin until every lane's target has published this sweep
 template <bool MULTI>
 __device__ __forceinline__ void coop_wait(const DevCtx& c, unsigned int tag, uint32_t tgt) {
@@ -251,7 +271,168 @@ __device__ __forceinline__ void coop_wait(const DevCtx& c, unsigned int tag, uin
     poll_backoff();
   }
   // acquire once: the word only grows, so this load reads a value >= tag and synchronises with its release
-  if (had) { if (remote) (void)ld_acquire_sys_u32(dp); else (void)ld_acquire_u32(dp); }
+  if (had) {
+    if (remote) (void)ld_acquire_sys_u32(dp); else (void)ld_acquire_u32(dp);
+#ifdef SM_AUDIT_HANDOFF
+    audit_acquired<MULTI>(c, tgt, tag);
+#endif
+  }
+}
+
+// Lane 0 publishes a step's hand-off: `done` (and `fin` under the exact schedule) with a release when somebody may wait
+// for it (`rel`), at system scope on a strip edge of a sharded map; otherwise a plain store.  Nobody waits for the latter,
+// and the release fence (the single most expensive instruction of a step: it waits for every write-back to be
+// acknowledged) is left to the sweep barrier.
+template <bool MULTI, bool EXACT>
+__device__ __forceinline__ void publish_handoff(const DevCtx& c, int pid, unsigned int tag, unsigned int pub, bool rel,
+                                                bool edge) {
+  if (rel) {
+    SM_AUDIT_RELEASED(c, pid, tag);
+    if (EXACT && !(MULTI && edge)) {      // one release fence for both words
+      fence_acq_rel_gpu();
+      st_relaxed_u32(&c.fin[pid], pub);
+      st_relaxed_u32(&c.done[pid], pub);
+    } else {
+      if (EXACT) st_release_u32(&c.fin[pid], pub);
+      if (MULTI && edge) st_release_sys_u32(&c.done[pid], pub);
+      else st_release_u32(&c.done[pid], pub);
+    }
+  } else {
+    if (EXACT) st_volatile_u32(&c.fin[pid], pub);
+    st_volatile_u32(&c.done[pid], pub);
+  }
+}
+
+// ---- wind: wait for exactly the lower-index particles in range (sm_handoff.cuh) -------------------------------
+// Bin b (0..8) of the 3x3 bins around (ix, iy): the head of its list for this sweep (SM_NIL: none), its nodes and the
+// rank tag of its owner.
+template <bool MULTI>
+__device__ __forceinline__ uint32_t wind_bin(const DevCtx& c, unsigned int tag, int b, int ix, int iy, const uint2*& nodes,
+                                             uint32_t& qtag) {
+  const int G = Reach<KIND_WIND>::G;
+  const int nbx = (c.dimx + G - 1) / G, nby = (c.dimy + G - 1) / G;
+  const int cx = ix / G + b / 3 - 1, cy = iy / G + b % 3 - 1;
+  if (cx < 0 || cx >= nbx || cy < 0 || cy >= nby) return SM_NIL;
+  const unsigned int par = tag & 1u;
+  const int bq = MULTI ? owner_of_x<MULTI>(c, cx * G) : 0;
+  const unsigned long long* hp = MULTI ? c.peer[bq].head[par] : c.head[par];
+  const unsigned long long h = *((volatile const unsigned long long*)&hp[cx * nby + cy]);
+  if ((unsigned int)(h >> 32) != tag) return SM_NIL;
+  nodes = MULTI ? c.peer[bq].node[par] : c.node[par];
+  qtag = MULTI ? ((uint32_t)bq << 28) : 0u;
+  return (uint32_t)h;
+}
+__device__ __forceinline__ bool wind_node_in_range(uint2 nd, int ix, int iy, int R) {
+  return handoff_in_range((int)(nd.y >> 18) - ix, (int)((nd.y >> 4) & 0x3FFFu) - iy, R, (int)(nd.y & 0xFu));
+}
+
+// Nine lanes walk the 3x3 bins and list every lower-index particle in range, up to SM_SW_NEARX of them (ws.cnt counts
+// them all, ws.pred[b] those of bin b); ws.succ = some higher-index particle in range, i.e. somebody waits for this one.
+// There is no own-bin predecessor and no per-bin fallback: every wait is a direct one, so only a particle that some
+// waiter lists has to release its hand-off.
+template <bool MULTI, bool EXACT>
+__device__ __forceinline__ void wind_scan(const DevCtx& c, WarpSmem& ws, int lane, unsigned int tag, int pid, int ix,
+                                          int iy, int R) {
+  if (lane == 0) { ws.cnt = 0; ws.succ = 0; if (EXACT) ws.remote = 0; }
+  if (EXACT && lane < SM_SW_NEARX / 32) ws.m0[lane] = 0;
+  __syncwarp();
+#ifdef SM_PROFILE
+  bool p_any = false, p_own_in = false;          // a higher index in the bins (the old succ); own-bin predecessor in range
+  uint32_t p_own = SM_NIL;                       // own-bin predecessor (lane 4)
+#endif
+  if (lane < 9) {
+    uint32_t mine = 0;
+    const uint2* nodes = nullptr;
+    uint32_t qtag = 0;
+    uint32_t j = wind_bin<MULTI>(c, tag, lane, ix, iy, nodes, qtag);
+    while (j != SM_NIL) {
+      const uint2 nd = nodes[j];
+      const bool in = wind_node_in_range(nd, ix, iy, R);
+#ifdef SM_PROFILE
+      if (j > (uint32_t)pid) p_any = true;
+      if (j < (uint32_t)pid && (p_own == SM_NIL || j > p_own)) { p_own = j; p_own_in = in; }
+#endif
+      if (in && j > (uint32_t)pid) ws.succ = 1u;            // (same value from every lane that sees one)
+      if (in && j < (uint32_t)pid) {
+        mine++;
+        const unsigned int at = atomicAdd(&ws.cnt, 1u);
+        if (at < SM_SW_NEARX) {
+          ws.blk[at] = j | qtag;
+          if (EXACT) {
+            ws.blkxy[at] = nd.y;
+            // static pruning: a neighbour whose box cannot meet plus(ipos) never delays the move
+            if (Foot<KIND_WIND>::box_hits_M((int)(nd.y >> 18) - ix, (int)((nd.y >> 4) & 0x3FFFu) - iy, (int)(nd.y & 0xFu)))
+              atomicOr(&ws.m0[at >> 5], 1u << (at & 31u));
+            if (MULTI && (qtag >> 28) != (uint32_t)c.rank) ws.remote = 1u;
+          }
+        }
+      }
+      j = nd.x;
+    }
+    ws.pred[lane] = mine;
+  }
+  __syncwarp();
+#ifdef SM_PROFILE
+  {   // row 16382 of the debug buffer: what the old and the new rule would fence and wait for
+    const bool any = __any_sync(0xffffffffu, p_any);
+    const uint32_t own = __shfl_sync(0xffffffffu, p_own, 4);
+    const bool own_in = __shfl_sync(0xffffffffu, p_own_in, 4);
+    if (lane == 0) {
+      unsigned long long* const h = c.dbg + 8 * 16382;
+      const unsigned int n = ws.cnt;
+      atomicAdd(&h[0], 1ull);                                     // scans
+      if (any) atomicAdd(&h[1], 1ull);                            // a higher index in the 3x3 bins (the old succ)
+      if (ws.succ) atomicAdd(&h[2], 1ull);                        // a higher index in range (the new succ)
+      if (own != SM_NIL) atomicAdd(&h[3], 1ull);                  // an own-bin predecessor exists
+      if (own != SM_NIL && !own_in) atomicAdd(&h[4], 1ull);       // ... and is out of range
+      atomicAdd(&h[n <= 31u ? 5 : (n <= SM_SW_NEARX ? 6 : 7)], 1ull);   // lower-index particles in range
+    }
+  }
+#endif
+}
+
+// Wait for every lower-index particle wind_scan found in range, 32 per round.  More than SM_SW_NEARX: the warp lists them
+// again in windows of SM_SW_NEARX, in a fixed order - bin lane, then bin-list order (the per-bin counts and their prefix
+// sum over the nine lanes give each entry its ordinal) - and polls one window after the other.  Every lane reaches every
+// coop_wait: the bin walks end at a __syncwarp before any lane polls, so no lane spins while another still walks a list.
+template <bool MULTI>
+__device__ __forceinline__ void wind_wait(const DevCtx& c, WarpSmem& ws, int lane, unsigned int tag, int pid, int ix,
+                                          int iy, int R) {
+  const unsigned int cnt = ws.cnt;
+  if (cnt <= SM_SW_NEARX) {
+    for (unsigned int base = 0; base < cnt; base += 32u)
+      coop_wait<MULTI>(c, tag, base + (unsigned int)lane < cnt ? ws.blk[base + lane] : SM_NIL);
+    return;
+  }
+  const unsigned int mine = lane < 9 ? ws.pred[lane] : 0u;
+  unsigned int first = mine;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const unsigned int v = __shfl_up_sync(0xffffffffu, first, o);
+    if (lane >= o) first += v;
+  }
+  first -= mine;                                  // ordinal of this bin's first entry
+  for (unsigned int win = 0; win < cnt; win += SM_SW_NEARX) {
+    __syncwarp();                                 // the previous window has been polled
+    if (mine != 0u && first < win + SM_SW_NEARX && first + mine > win) {
+      const uint2* nodes = nullptr;
+      uint32_t qtag = 0;
+      uint32_t j = wind_bin<MULTI>(c, tag, lane, ix, iy, nodes, qtag);
+      unsigned int ord = first;
+      while (j != SM_NIL && ord < win + SM_SW_NEARX) {
+        const uint2 nd = nodes[j];
+        if (j < (uint32_t)pid && wind_node_in_range(nd, ix, iy, R)) {
+          if (ord >= win) ws.blk[ord - win] = j | qtag;
+          ord++;
+        }
+        j = nd.x;
+      }
+    }
+    __syncwarp();
+    const unsigned int m = cnt - win < SM_SW_NEARX ? cnt - win : SM_SW_NEARX;
+    for (unsigned int base = 0; base < m; base += 32u)
+      coop_wait<MULTI>(c, tag, base + (unsigned int)lane < m ? ws.blk[base + lane] : SM_NIL);
+  }
 }
 
 // ---- barrier across the blocks of every rank of a sharded map ---------------------------------------------
@@ -317,7 +498,8 @@ __device__ __forceinline__ unsigned int grid_barrier_x(const DevCtx& c, unsigned
 // footprints do not.  With EXACT a
 // particle publishes three words per sweep: mv (= npos, right after move(); it only lets others SKIP a wait, so it
 // needs no fence), fin (its map writes are complete; release) and done (published in own-bin index order, which
-// keeps "X done => every lower index in X's bin done" and with it the crowded fallback sound).  A lower-index
+// keeps "X done => every lower index in X's bin done" and with it the crowded fallback sound; wind on one rank waits
+// for particles in range only and publishes both words together).  A lower-index
 // particle B in range holds A back
 //   before A.move()     only while B's writes {ipos_B} U 3x3(npos_B) can meet plus(ipos_A)
 //                       (B not moved yet: while B's box can),
@@ -367,7 +549,12 @@ __device__ __forceinline__ int sweep_exact(const DevCtx& c, WarpSmem& ws, WarpDe
       if (!__any_sync(0xffffffffu, need0)) break;
       poll_backoff();
     }
-    if (acq) (void)ld_acquire_u32(&c.fin[j]);
+    if (acq) {
+      (void)ld_acquire_u32(&c.fin[j]);
+#ifdef SM_AUDIT_HANDOFF
+      audit_acquired<false>(c, j, tag);
+#endif
+    }
     const unsigned int left = __ballot_sync(0xffffffffu, need1);
     if (lane == 0) ws.n1[base >> 5] = left;
   }
@@ -407,15 +594,24 @@ __device__ __forceinline__ int sweep_exact(const DevCtx& c, WarpSmem& ws, WarpDe
         if (!__any_sync(0xffffffffu, need1)) break;
         poll_backoff();
       }
-      if (acq) (void)ld_acquire_u32(&c.fin[j]);
+      if (acq) {
+        (void)ld_acquire_u32(&c.fin[j]);
+#ifdef SM_AUDIT_HANDOFF
+        audit_acquired<false>(c, j, tag);
+#endif
+      }
     }
     r = do_interact_coop(w, a, p, mid);
     a.flush(w);
   }
   // stalled or left the map in move(): only track[] was written
-  if (lane == 0) {
+  if constexpr (KIND == KIND_WIND && !MULTI) {
+    // no ordered `done`: the conservative wind path waits for particles in range only (wind_wait)
+    if (lane == 0) publish_handoff<MULTI, true>(c, pid, tag, (r == SM_ALIVE) ? tag : 0xFFFFFFFFu, ws.succ != 0u, edge);
+  } else if (lane == 0) {
     const unsigned int pub = (r == SM_ALIVE) ? tag : 0xFFFFFFFFu;
     if (ws.succ) {
+      SM_AUDIT_RELEASED(c, pid, tag);
       // `done` in own-bin index order
       const unsigned int* dp = nullptr;
       if (ownpred != SM_NIL) dp = MULTI ? &c.peer[ownpred >> 28].done[ownpred & 0x0FFFFFFFu] : &c.done[ownpred];
@@ -627,7 +823,10 @@ __global__ void __launch_bounds__(SwShape<KIND>::WARPS * 32, SwShape<KIND>::MINB
       load_particle(c, pid, p);
       const int ix = (int)roundf(p.px), iy = (int)roundf(p.py);
       const int myR = particle_reach(p);
-      const uint32_t tgt = coop_scan<KIND, MULTI, EXACT>(c, ws, lane, tag, pid, ix, iy, myR);
+      uint32_t tgt = SM_NIL;
+      // wind on one rank: the in-range rule of sm_handoff.cuh; sharded maps keep the own-bin order for now
+      if constexpr (KIND == KIND_WIND && !MULTI) wind_scan<MULTI, EXACT>(c, ws, lane, tag, pid, ix, iy, myR);
+      else tgt = coop_scan<KIND, MULTI, EXACT>(c, ws, lane, tag, pid, ix, iy, myR);
 #ifdef SM_PROFILE
       const long long pc1 = clock64();
       long long pc2 = pc1;
@@ -648,7 +847,8 @@ __global__ void __launch_bounds__(SwShape<KIND>::WARPS * 32, SwShape<KIND>::MINB
         if (exact_now) r = sweep_exact<KIND, MULTI, BUDGET, CELLS>(c, ws, w, s_soils, tag, pid, ix, iy, myR, p, edge, &cm);
       }
       if (!exact_now) {
-        coop_wait<MULTI>(c, tag, tgt);
+        if constexpr (KIND == KIND_WIND && !MULTI) wind_wait<MULTI>(c, ws, lane, tag, pid, ix, iy, myR);
+        else coop_wait<MULTI>(c, tag, tgt);
 #ifdef SM_PROFILE
         pc2 = clock64();
 #endif
@@ -668,26 +868,9 @@ __global__ void __launch_bounds__(SwShape<KIND>::WARPS * 32, SwShape<KIND>::MINB
 #endif
         // hand-off first: the map writes are all the successors of this step wait for
         a.flush(w);
-        if (lane == 0) {
-          const unsigned int pub = (r == SM_ALIVE) ? tag : 0xFFFFFFFFu;
-          if (ws.succ) {
-            if (EXACT && !(MULTI && edge)) {      // one release fence for both words
-              fence_acq_rel_gpu();
-              st_relaxed_u32(&c.fin[pid], pub);
-              st_relaxed_u32(&c.done[pid], pub);
-            } else {
-              if (EXACT) st_release_u32(&c.fin[pid], pub);
-              if (MULTI && edge) st_release_sys_u32(&c.done[pid], pub);
-              else st_release_u32(&c.done[pid], pub);
-            }
-          } else {
-            // Nobody can be waiting for this hand-off: a waiter lists particles of its own 3x3 bins, so it would
-            // sit in ours, and no higher index does.  The release fence (the single most expensive instruction of
-            // a step: it waits for every write-back to be acknowledged) is left to the sweep barrier.
-            if (EXACT) st_volatile_u32(&c.fin[pid], pub);
-            st_volatile_u32(&c.done[pid], pub);
-          }
-        }
+        // water: a waiter lists particles of its own 3x3 bins, so with no higher index in ours nobody waits for this
+        // hand-off; wind: nobody in range does (sm_handoff.cuh)
+        if (lane == 0) publish_handoff<MULTI, EXACT>(c, pid, tag, (r == SM_ALIVE) ? tag : 0xFFFFFFFFu, ws.succ != 0u, edge);
 #ifdef SM_PROFILE
         if (lane == 0) {   // phase sums of the conservative path, row 16383 of the debug buffer
           const long long pcp = clock64();
