@@ -249,6 +249,23 @@ class Layermap {
     return out;
   }
 
+  // How the map drains, in one read-only call (sm_drainage; ground: SM_DRAIN_GROUND, the ground under standing
+  // water).  Rasters in cell order x*dim.y + y: the spill height, the receiver's index into the neighbour order
+  // (-1 on the border), the cells draining through each cell, and the border cell each drains to (x*dim.y + y).
+  struct Drainage {
+    std::vector<double> spill;
+    std::vector<int8_t> dir;
+    std::vector<int64_t> area, basin;
+    sm_drain_stats stats;
+  };
+  Drainage drainage(bool ground = false) {
+    const size_t n = (size_t)dim.x * (size_t)dim.y;
+    Drainage d{std::vector<double>(n), std::vector<int8_t>(n), std::vector<int64_t>(n), std::vector<int64_t>(n), {}};
+    ck(sm_drainage(ctx, ground ? SM_DRAIN_GROUND : 0, d.spill.data(), d.dir.data(), d.area.data(), d.basin.data(), 0,
+                   &d.stats));
+    return d;
+  }
+
   // ---- meshing (layermap.h:443-555) --------------------------------------------------------------------------
   // The renderer's vertex pool is outside the boundary; what crosses it is the vertex data.  update(vp) meshes
   // the whole map on the device (one 44-byte Vertex {position[3], normal[3], color[4], index} per cell, cell order

@@ -110,6 +110,8 @@ int sm_sync(sm_context* ctx);
  * each of its phases needs every rank's previous phase, a barrier across processes per phase; a group offers it.
  * sm_composition and sm_voxelize read a rank's own strip (same precondition; a voxel window must lie inside the strip):
  * each rank reads its own part and the caller joins the parts.
+ * sm_drainage on a rank computes the whole map on the rank's device through the peer pointers (same precondition) and
+ * writes the rank's strip; every rank that calls it repeats the whole-map work.
  * sm_peer_attach with use_ipc = 0 enables peer access to a blob's device when it differs from the context's. */
 #define SM_PEER_ARRAYS 23
 #define SM_PEER_SLOTS 24
@@ -157,6 +159,7 @@ int sm_hydro_issuer(sm_context* ctx, int32_t on);
  *   sm_peer_export, sm_peer_attach, sm_hydro_issuer: SM_ERR_INVALID (the group manages its ranks).
  *   sm_composition, sm_voxelize: every rank computes its slice of the whole-map planes after every rank's work has
  *     completed; device output lands in rank 0's buffer; the counts are summed, device_ms is the slowest rank's.
+ *   sm_drainage: rank 0 computes the whole map after every rank's work has completed, into the caller's buffers.
  * The group waits for every rank (sm_sync on each) before a call that reads or writes other ranks' strips, and only
  * when something was enqueued since the last wait.  SM_FLAG_BUDGET and SM_FLAG_CELL_BUDGET pass through to the ranks;
  * SM_FLAG_HYDRO_CELL_BUDGET with nranks > 1 is refused as by sm_create_sharded.  pool_capacity == 0 keeps the sharded
@@ -381,6 +384,63 @@ int sm_composition(sm_context* ctx, const int32_t* types, int32_t ntypes, double
                    double* out, int32_t on_device, sm_view_stats* stats);
 int sm_voxelize(sm_context* ctx, int32_t x0, int32_t x1, int32_t y0, int32_t y1, double z0, double dz, int32_t nz,
                 uint8_t* out, int32_t on_device, sm_view_stats* stats);
+
+/* ---- drainage: how the map drains, in one call (DESIGN.md section 14) -----------------------------------------------
+ * Definitions (cell order x*dimy + y, like every other raster):
+ *   H(c), the height of cell c: without flags, what sm_download_height returns: top.floor + top.size, or 0.0 for an
+ *     empty column.  With SM_DRAIN_GROUND, the ground under standing water: floor + size of the first section met
+ *     walking top -> bottom whose type is not Air (type 0), or 0.0 if there is none (the chain walk of the strata views).
+ *   Border cells are those with x in {0, dimx - 1} or y in {0, dimy - 1}.  They are the outlets: water leaves the map
+ *     there.
+ *   spill W(c): the minimum, over all 8-connected paths from c to a border cell, of the largest H on the path, c
+ *     included.  Equivalently, W is the unique solution of W = H on border cells and W(c) = max(H(c), min over the 8
+ *     neighbours W(n)) inside.  The cell's depression depth is W - H: one subtraction, bit-exact against the same H.
+ *     W uses only min and max, so it is exact in f64 in any evaluation order.
+ *   dir(c): an index k into the neighbour order n[] = (-1,-1), (-1,0), (-1,1), (0,-1), (0,1), (1,-1), (1,0), (1,1)
+ *     of (dx, dy).  Rules, in order:
+ *     -1 on a border cell.
+ *     A drained cell has a neighbour with W(n) < W(c).  Its dir is the k of largest (W(c) - W(n)) / d, with d = 1.0 or
+ *     sqrt(2.0) (f64, correctly rounded).  Ties go to the lower k.
+ *     Any other interior cell lies on a flat.  dist(c) is the number of 8-connected steps through cells of equal W to
+ *     the nearest drained or border cell of that W.  The flat cell's dir is the lowest k with W(n) == W(c) and
+ *     dist(n) == dist(c) - 1.
+ *     After filling, such an n always exists.  The receivers form a forest rooted at the border cells: each hop lowers
+ *     W, or keeps W and lowers dist.
+ *   area(c) = 1 + the sum of area(d) over every d whose receiver is c: the cells that drain through c, itself
+ *     included.  An exact int64.
+ *   basin(c) = the global index x*dimy + y of the border cell at which c's receiver chain ends.
+ * Any of spill, dir, area, basin may be NULL: that output is then not written, but it is still computed when a later
+ * output needs it.  flags: SM_DRAIN_GROUND, no other bit.  on_device != 0: the outputs are device pointers on the
+ * context's device (rank 0's for a group); otherwise host memory.  stats may be NULL.
+ * The call is read-only: columns, pool, frequency arrays, budgets and per-cell maps, the mesh and an open batch are left
+ * exactly as they were.  A refusal (an unknown flag bit, all four outputs NULL, no map: a rank of a sharded map
+ * without its peers attached) returns SM_ERR_INVALID before any launch, with nothing written.
+ * The view is global: a cell's spill height can depend on the far side of the map, so every computation runs over the
+ * whole map on one device, which first gathers H of every strip into a whole-map raster.  It needs about 50 B per cell
+ * of device memory there (about 3.4 GB at 8192^2), freed when the call returns.  Group: rank 0 computes after every
+ * rank's work has completed, and the results go into the caller's whole-map buffers.  Rank of a sharded map (in
+ * process or across processes over CUDA IPC): it needs sm_peer_attach and the precondition of the views above (every
+ * rank's earlier work has completed); the rank computes the whole map and writes its own strip, in cell order
+ * (x - x0)*dimy + y, with basin still holding global indices.  Each rank that calls it repeats the whole-map work.
+ * Every output is byte for byte that of one context.
+ * Stats: fill_passes and dist_passes are the tile passes of the two relaxations, up to the one that changed nothing;
+ * with tiles racing in one pass they can differ from run to run, the results cannot.  jump_passes: the pointer-jumping
+ * passes of the basins.  longest_walk: the most receivers one walker of the area phase visited.  phase_ms: CUDA-event
+ * time of heights, fill, dist, receivers, area, basin; device_ms is their sum. */
+#define SM_DRAIN_GROUND 1
+typedef struct sm_drain_stats {
+  int64_t fill_passes;      /* tile passes of the fill */
+  int64_t flat_cells;       /* interior cells that are not drained */
+  int64_t depressed_cells;  /* cells with W > H */
+  int64_t outlets;          /* border cells with area > 1 */
+  double device_ms;         /* CUDA-event time of the kernels */
+  int64_t dist_passes;      /* tile passes of the flat distances */
+  int64_t jump_passes;      /* pointer-jumping passes of the basins */
+  int64_t longest_walk;     /* receivers visited by the longest area walker */
+  double phase_ms[6];       /* heights, fill, dist, receivers, area, basin */
+} sm_drain_stats;
+int sm_drainage(sm_context* ctx, int32_t flags, double* spill, int8_t* dir, int64_t* area, int64_t* basin,
+                int32_t on_device, sm_drain_stats* stats);
 
 /* WaterParticle::frequency/track, WindParticle::frequency (water.h:345-346, wind.h:48).
  * Any pointer may be NULL. */

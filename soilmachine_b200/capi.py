@@ -41,7 +41,7 @@ SYMBOLS = [
     "sm_create_group", "sm_group_size", "sm_group_rank", "sm_group_layout",
     "sm_snapshot_bytes", "sm_snapshot_save", "sm_snapshot_restore",
     "sm_apply_layer", "sm_relax", "sm_composition", "sm_voxelize",
-    "sm_water_run_flooding",
+    "sm_water_run_flooding", "sm_drainage",
 ]
 
 
@@ -113,6 +113,22 @@ SM_COMP_BELOW_SURFACE = 1
 SM_COMP_PORE_WATER = 2
 SM_VOXEL_NONE = 255
 SM_VOXEL_MAX_NZ = 65536
+
+
+class DrainStats(C.Structure):
+    _fields_ = [("fill_passes", C.c_int64), ("flat_cells", C.c_int64), ("depressed_cells", C.c_int64),
+                ("outlets", C.c_int64), ("device_ms", C.c_double), ("dist_passes", C.c_int64),
+                ("jump_passes", C.c_int64), ("longest_walk", C.c_int64), ("phase_ms", C.c_double * 6)]
+    PHASES = ("heights", "fill", "dist", "receivers", "area", "basin")
+
+    def asdict(self):
+        d = {k: getattr(self, k) for k, _ in self._fields_ if k != "phase_ms"}
+        d["phase_ms"] = dict(zip(self.PHASES, list(self.phase_ms)))
+        return d
+
+
+SM_DRAIN_GROUND = 1
+DRAIN_OUTPUTS = (("spill", np.float64), ("dir", np.int8), ("area", np.int64), ("basin", np.int64))
 
 
 CELL_TERMS = ("eroded", "deposited", "cascade_net")     # sm_last_cell_budget
@@ -442,6 +458,29 @@ class Context:
         self._ck_strict(self.lib.sm_voxelize(self.h, int(x0), int(x1), int(y0), int(y1), C.c_double(z0), C.c_double(dz),
                                              int(nz), ptr, dev, C.byref(st)))
         self.view_stats = st
+        return res
+
+    # ---- drainage -------------------------------------------------------------------------------------------------
+    def drainage(self, ground=False, out=None, outputs=("spill", "dir", "area", "basin")):
+        """sm_drainage: how the map drains.  Returns a dict of (x1 - x0, dimy) arrays - the whole map, or this rank's
+        strip of a sharded map: spill (float64, the spill height W), dir (int8, the receiver's index into the
+        neighbour order, -1 on the border), area (int64, the cells draining through the cell) and basin (int64, the
+        global index of the border cell the cell drains to), for the names in `outputs`.  ground=True reads the
+        ground under standing water instead of the top of the column.  out: a dict of device pointers (device_alloc,
+        this many cells each) to write instead of host arrays; then returns None.  The call's DrainStats are kept in
+        self.drain_stats.  A refusal raises with nothing written."""
+        st = DrainStats()
+        ptrs, res = {}, None
+        if out is None:
+            res = {k: np.empty((self.x1 - self.x0, self.dimy), t) for k, t in DRAIN_OUTPUTS if k in outputs}
+            ptrs = {k: v.ctypes.data_as(C.c_void_p) for k, v in res.items()}
+            dev = 0
+        else:
+            ptrs = {k: C.c_void_p(v.value if isinstance(v, C.c_void_p) else v) for k, v in out.items() if v is not None}
+            dev = 1
+        self._ck_strict(self.lib.sm_drainage(self.h, SM_DRAIN_GROUND if ground else 0, ptrs.get("spill"), ptrs.get("dir"),
+                                             ptrs.get("area"), ptrs.get("basin"), dev, C.byref(st)))
+        self.drain_stats = st
         return res
 
     def set_soil_colors(self, rgba):

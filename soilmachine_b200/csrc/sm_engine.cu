@@ -24,6 +24,7 @@
 #include "sm_layer.cuh"
 #include "sm_relax.cuh"
 #include "sm_strata.cuh"
+#include "sm_drain.cuh"
 #include <cub/device/device_scan.cuh>
 #include <type_traits>
 
@@ -4020,6 +4021,425 @@ int sm_voxelize(sm_context* ctx, int32_t x0, int32_t x1, int32_t y0, int32_t y1,
     st.device_ms = std::max(st.device_ms, part.device_ms);
   }
   if (ctx->group) ctx->group->dirty = false;
+  if (stats) *stats = st;
+  return SM_OK;
+}
+
+}  // extern "C"
+
+// ---- drainage (sm_drain.cuh, DESIGN.md section 14) ------------------------------------------------------------------
+// Every phase works on whole-map rasters in cell order x*dimy + y on the computing device.  The two relaxations run on
+// tiles of DRAIN_T x DRAIN_T cells: a block loads its tile and a one-cell halo into shared memory, relaxes it to local
+// stability, writes back what changed and marks for the next pass the neighbour tiles whose halo it changed.
+#define DRAIN_T 32
+#define DRAIN_S (DRAIN_T + 2)
+#define DRAIN_BATCH 4          // relaxation passes launched between two reads of their mark counters
+
+// H of every cell of the whole map, each column read from its owner (MULTI: through the peer pointers); the fill
+// starts from W = H on the border, +inf inside.
+template <bool MULTI>
+__global__ void __launch_bounds__(256) k_drain_heights(DevCtx c, int ground, double* __restrict__ H, double* __restrict__ W) {
+  const size_t n = (size_t)c.dimx * c.dimy;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    const int x = (int)(i / (size_t)c.dimy), y = (int)(i % (size_t)c.dimy);
+    const StrataPool a{MULTI ? c.peer[owner_of_x<MULTI>(c, x)].pool : c.pool};
+    const double h = drain_column_height(a, *cell_ptr<MULTI>(c, x, y), ground != 0);
+    H[i] = h;
+    W[i] = (x == 0 || y == 0 || x == c.dimx - 1 || y == c.dimy - 1) ? h : (double)INFINITY;
+  }
+}
+
+// One pass of a tiled relaxation.  DIST = false: the fill, W(c) = max(H(c), min_n W(n)) on interior cells.  DIST =
+// true: the flat distances, on cells whose D is not SM_DRAIN_NOT_FLAT.  Tile t runs when act_cur[t] is set and clears
+// it; *marks counts the tiles it sets in act_next.
+template <bool DIST>
+__global__ void __launch_bounds__(256) k_drain_relax(const double* __restrict__ H, double* W, int32_t* D, int dimx, int dimy,
+                                                     int ntx, int nty, unsigned int* act_cur, unsigned int* act_next,
+                                                     unsigned long long* marks) {
+  __shared__ double sw[DRAIN_S][DRAIN_S];
+  __shared__ int32_t sd[DIST ? DRAIN_S : 1][DIST ? DRAIN_S : 1];
+  __shared__ unsigned int s_on, s_dirs;
+  const int tile = blockIdx.x, tid = threadIdx.y * DRAIN_T + threadIdx.x;
+  if (tid == 0) {
+    s_on = act_cur[tile];
+    if (s_on) act_cur[tile] = 0;
+    s_dirs = 0;
+  }
+  __syncthreads();
+  if (!s_on) return;
+  const int TX = tile / nty, TY = tile % nty, X0 = TX * DRAIN_T, Y0 = TY * DRAIN_T;
+  for (int i = tid; i < DRAIN_S * DRAIN_S; i += blockDim.x * blockDim.y) {
+    const int lx = i / DRAIN_S, ly = i % DRAIN_S, gx = X0 - 1 + lx, gy = Y0 - 1 + ly;
+    const bool in = gx >= 0 && gx < dimx && gy >= 0 && gy < dimy;
+    const size_t g = (size_t)gx * dimy + gy;
+    sw[lx][ly] = in ? W[g] : (double)INFINITY;
+    if (DIST) sd[DIST ? lx : 0][DIST ? ly : 0] = in ? D[g] : SM_DRAIN_FAR;
+  }
+  __syncthreads();
+  constexpr int R = DRAIN_T * DRAIN_T / 256;
+  double h[R];
+  bool live[R];
+  const int ly = threadIdx.x, Y = Y0 + ly;
+#pragma unroll
+  for (int j = 0; j < R; j++) {
+    const int lx = threadIdx.y + j * (256 / DRAIN_T), X = X0 + lx;
+    live[j] = X > 0 && X < dimx - 1 && Y > 0 && Y < dimy - 1;
+    if (DIST) live[j] = live[j] && sd[DIST ? lx + 1 : 0][DIST ? ly + 1 : 0] != SM_DRAIN_NOT_FLAT;
+    h[j] = !live[j] ? 0.0 : (DIST ? sw[lx + 1][ly + 1] : H[(size_t)X * dimy + Y]);
+  }
+  bool mine = false;
+  SM_UNROLL1
+  for (;;) {
+    bool ch = false;
+#pragma unroll
+    for (int j = 0; j < R; j++) {
+      if (!live[j]) continue;
+      const int lx = threadIdx.y + j * (256 / DRAIN_T) + 1, cy = ly + 1;
+      double wn[8];
+#pragma unroll
+      for (int k = 0; k < 8; k++) wn[k] = sw[lx + drain_dx(k)][cy + drain_dy(k)];
+      if (!DIST) {
+        const double v = drain_fill_value(h[j], wn);
+        if (v < sw[lx][cy]) { sw[lx][cy] = v; ch = true; }
+      } else {
+        int32_t dn[8];
+#pragma unroll
+        for (int k = 0; k < 8; k++) dn[k] = sd[DIST ? lx + drain_dx(k) : 0][DIST ? cy + drain_dy(k) : 0];
+        const int32_t dc = sd[DIST ? lx : 0][DIST ? cy : 0];
+        const int32_t v = drain_dist_value(h[j], dc, wn, dn);
+        if (v < dc) { sd[DIST ? lx : 0][DIST ? cy : 0] = v; ch = true; }
+      }
+    }
+    mine |= ch;
+    if (!__syncthreads_or(ch)) break;
+  }
+  if (mine) {       // write back what changed; the neighbour tiles whose halo holds a changed cell run again
+    unsigned int dirs = 0;
+#pragma unroll
+    for (int j = 0; j < R; j++) {
+      if (!live[j]) continue;
+      const int lx = threadIdx.y + j * (256 / DRAIN_T);
+      const size_t g = (size_t)(X0 + lx) * dimy + Y;
+      bool changed;
+      if (!DIST) {
+        changed = sw[lx + 1][ly + 1] != W[g];
+        if (changed) W[g] = sw[lx + 1][ly + 1];
+      } else {
+        const int32_t v = sd[DIST ? lx + 1 : 0][DIST ? ly + 1 : 0];
+        changed = v != D[g];
+        if (changed) D[g] = v;
+      }
+      if (!changed) continue;
+      const int ax = lx == 0 ? -1 : 0, bx = lx == DRAIN_T - 1 ? 1 : 0;
+      const int ay = ly == 0 ? -1 : 0, by = ly == DRAIN_T - 1 ? 1 : 0;
+      for (int dx = ax; dx <= bx; dx++)
+        for (int dy = ay; dy <= by; dy++)
+          if (dx || dy) dirs |= 1u << ((dx + 1) * 3 + (dy + 1));
+    }
+    if (dirs) atomicOr(&s_dirs, dirs);
+  }
+  __syncthreads();
+  if (tid == 0 && s_dirs) {
+    unsigned long long n = 0;
+    for (int b = 0; b < 9; b++) {
+      if (!(s_dirs & (1u << b))) continue;
+      const int tx = TX + b / 3 - 1, ty = TY + b % 3 - 1;
+      if (tx < 0 || tx >= ntx || ty < 0 || ty >= nty) continue;
+      act_next[tx * nty + ty] = 1u;
+      n++;
+    }
+    if (n) atomicAdd(marks, n);
+  }
+}
+
+// the 3x3 window of a whole-map raster around the interior cell (x, y), neighbours in the order n[k]
+template <class T>
+__device__ __forceinline__ void drain_window(const T* __restrict__ a, int x, int y, int dimy, T* out) {
+#pragma unroll
+  for (int k = 0; k < 8; k++) out[k] = a[(size_t)(x + drain_dx(k)) * dimy + (y + drain_dy(k))];
+}
+__device__ __forceinline__ bool drain_border(int x, int y, int dimx, int dimy) {
+  return x == 0 || y == 0 || x == dimx - 1 || y == dimy - 1;
+}
+
+// after the fill: D = SM_DRAIN_NOT_FLAT on drained and border cells, SM_DRAIN_FAR on flat ones.  cnt[0] += flat
+// cells, cnt[1] += cells with W > H.
+__global__ void __launch_bounds__(256) k_drain_classify(const double* __restrict__ H, const double* __restrict__ W,
+                                                        int32_t* __restrict__ D, int dimx, int dimy,
+                                                        unsigned long long* __restrict__ cnt) {
+  const size_t n = (size_t)dimx * dimy;
+  unsigned long long flat = 0, dep = 0;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    const int x = (int)(i / (size_t)dimy), y = (int)(i % (size_t)dimy);
+    bool f = false;
+    if (!drain_border(x, y, dimx, dimy)) {
+      double wn[8];
+      drain_window(W, x, y, dimy, wn);
+      f = !drain_drained(W[i], wn);
+    }
+    D[i] = f ? SM_DRAIN_FAR : SM_DRAIN_NOT_FLAT;
+    flat += f;
+    dep += W[i] > H[i];
+  }
+  block_add_u64(flat, &cnt[0]);
+  block_add_u64(dep, &cnt[1]);
+}
+
+// receivers: dir (k or -1), rcv (the receiver's cell or -1), in-degrees, area = 1 (area may be null).  cnt[2] +=
+// interior cells without a receiver (none at the fixed point).
+__global__ void __launch_bounds__(256) k_drain_receivers(const double* __restrict__ W, const int32_t* __restrict__ D,
+                                                         int dimx, int dimy, int8_t* __restrict__ dir, int32_t* __restrict__ rcv,
+                                                         int32_t* indeg, unsigned long long* __restrict__ area,
+                                                         unsigned long long* __restrict__ cnt) {
+  const size_t n = (size_t)dimx * dimy;
+  unsigned long long bad = 0;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    const int x = (int)(i / (size_t)dimy), y = (int)(i % (size_t)dimy);
+    int k = -1;
+    if (!drain_border(x, y, dimx, dimy)) {
+      double wn[8];
+      int32_t dn[8];
+      drain_window(W, x, y, dimy, wn);
+      drain_window(D, x, y, dimy, dn);
+      k = drain_receiver(W[i], D[i], wn, dn);
+      bad += k < 0;
+    }
+    dir[i] = (int8_t)k;
+    if (area) area[i] = 1ull;
+    if (k < 0) {
+      rcv[i] = -1;
+    } else {
+      const int r = (x + drain_dx(k)) * dimy + (y + drain_dy(k));
+      rcv[i] = r;
+      atomicAdd(&indeg[r], 1);
+    }
+  }
+  block_add_u64(bad, &cnt[2]);
+}
+
+// cnt[3] += border cells with a donor (area > 1)
+__global__ void __launch_bounds__(256) k_drain_outlets(const int32_t* __restrict__ indeg, int dimx, int dimy,
+                                                       unsigned long long* __restrict__ cnt) {
+  const size_t n = (size_t)dimx * dimy;
+  unsigned long long o = 0;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    const int x = (int)(i / (size_t)dimy), y = (int)(i % (size_t)dimy);
+    o += drain_border(x, y, dimx, dimy) && indeg[i] > 0;
+  }
+  block_add_u64(o, &cnt[3]);
+}
+
+// Upstream area: one walker per cell without donors carries its area downstream.  At each receiver it adds its area,
+// fences, and takes one from rem (a copy of the in-degrees); the walker that takes the last one owns the receiver's
+// complete area and goes on from there.  Every cell is passed on exactly once, with integer sums.  *longest = the
+// most receivers one walker visited.
+__global__ void __launch_bounds__(256) k_drain_area(const int32_t* __restrict__ rcv, const int32_t* __restrict__ indeg,
+                                                    int32_t* rem, unsigned long long* area, size_t n,
+                                                    unsigned long long* __restrict__ longest) {
+  unsigned long long most = 0;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    if (indeg[i] != 0) continue;
+    unsigned long long a = 1ull, hops = 0;
+    int32_t r = rcv[i];
+    SM_UNROLL1
+    while (r >= 0) {
+      atomicAdd(&area[r], a);
+      __threadfence();
+      hops++;
+      if (atomicSub(&rem[r], 1) != 1) break;
+      __threadfence();
+      a = atomicAdd(&area[r], 0ull);
+      r = rcv[r];
+    }
+    most = hops > most ? hops : most;
+  }
+  if (most) atomicMax(longest, most);
+}
+
+// basins: nxt = the receiver, or the cell itself on the border; then jumps nxt = nxt[nxt] until nothing changes
+__global__ void __launch_bounds__(256) k_drain_basin_init(const int32_t* __restrict__ rcv, int32_t* __restrict__ nxt, size_t n) {
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
+    nxt[i] = rcv[i] < 0 ? (int32_t)i : rcv[i];
+}
+__global__ void __launch_bounds__(256) k_drain_jump(int32_t* nxt, size_t n, unsigned long long* __restrict__ changed) {
+  unsigned long long c = 0;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    const int32_t a = nxt[i], b = nxt[a];
+    if (a != b) { nxt[i] = b; c++; }
+  }
+  block_add_u64(c, changed);
+}
+// basin[i] = nxt[i] as int64, cells [c0, c0 + m)
+__global__ void __launch_bounds__(256) k_drain_basin_out(const int32_t* __restrict__ nxt, size_t c0, size_t m,
+                                                         int64_t* __restrict__ out) {
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < m; i += (size_t)gridDim.x * blockDim.x)
+    out[i] = (int64_t)nxt[c0 + i];
+}
+
+namespace {
+struct DrainTimer {        // CUDA-event time of each phase's launches, summed per phase
+  StrataEvents e;
+  double ms[6] = {};
+};
+// the counters of one call, in one device array
+enum { DC_FLAT, DC_DEPRESSED, DC_BAD, DC_OUTLETS, DC_LONGEST, DC_JUMP, DC_MARKS = 8, DC_N = DC_MARKS + DRAIN_BATCH };
+}  // namespace
+
+// One tiled relaxation, pass after pass until a pass marks no tile.  Returns the passes.
+template <bool DIST>
+static int drain_relax(sm_context* ctx, DrainTimer& tm, int phase, const double* H, double* W, int32_t* D,
+                       unsigned int* act, unsigned long long* d_marks, int64_t* passes) {
+  const int dimx = ctx->d.dimx, dimy = ctx->d.dimy;
+  const int ntx = (dimx + DRAIN_T - 1) / DRAIN_T, nty = (dimy + DRAIN_T - 1) / DRAIN_T;
+  const size_t nt = (size_t)ntx * nty;
+  std::vector<unsigned int> ones(nt, 1u);
+  CK(cudaMemcpyAsync(act, ones.data(), nt * 4, cudaMemcpyHostToDevice, ctx->stream));
+  CK(cudaMemsetAsync(act + nt, 0, nt * 4, ctx->stream));
+  unsigned long long h_marks[DRAIN_BATCH];
+  *passes = 0;
+  for (int64_t p = 0;; p += DRAIN_BATCH) {
+    CK(cudaMemsetAsync(d_marks, 0, sizeof(h_marks), ctx->stream));
+    CK(cudaEventRecord(tm.e.e0, ctx->stream));
+    for (int b = 0; b < DRAIN_BATCH; b++) {
+      const int64_t q = p + b;
+      k_drain_relax<DIST><<<(unsigned)nt, dim3(DRAIN_T, 256 / DRAIN_T), 0, ctx->stream>>>(
+          H, W, D, dimx, dimy, ntx, nty, act + (q & 1) * nt, act + ((q + 1) & 1) * nt, d_marks + b);
+      ctx->launches++;
+    }
+    CK(cudaGetLastError());
+    CK(cudaEventRecord(tm.e.e1, ctx->stream));
+    CK(cudaMemcpyAsync(h_marks, d_marks, sizeof(h_marks), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    float m = 0.f;
+    CK(cudaEventElapsedTime(&m, tm.e.e0, tm.e.e1));
+    tm.ms[phase] += m;
+    for (int b = 0; b < DRAIN_BATCH; b++) {
+      ++*passes;
+      if (h_marks[b] == 0) return SM_OK;
+    }
+  }
+}
+
+extern "C" {
+
+int sm_drainage(sm_context* ctx, int32_t flags, double* spill, int8_t* dir, int64_t* area, int64_t* basin,
+                int32_t on_device, sm_drain_stats* stats) {
+  if (flags & ~SM_DRAIN_GROUND) return fail(ctx, SM_ERR_INVALID, "sm_drainage: unknown flags");
+  if (!spill && !dir && !area && !basin) return fail(ctx, SM_ERR_INVALID, "sm_drainage: no output requested");
+  int rc;
+  sm_context* c = ctx;       // the computing context: rank 0 of a group
+  if (ctx->group) {
+    if ((rc = grp_settle(ctx)) != SM_OK) return rc;
+    c = ctx->group->rank[0];
+  } else if ((rc = peers_ready(ctx)) != SM_OK) {
+    return rc;
+  }
+  const bool multi = c->nranks > 1;
+  const int dimx = c->d.dimx, dimy = c->d.dimy;
+  const size_t N = (size_t)dimx * dimy;
+  // the cells this call writes: the whole map, or a rank's strip
+  const size_t c0 = ctx->group ? 0 : (size_t)c->x0 * dimy, m = ctx->group ? N : c->lcells;
+  const bool want_rcv = dir || area || basin;
+  const int ntx = (dimx + DRAIN_T - 1) / DRAIN_T, nty = (dimy + DRAIN_T - 1) / DRAIN_T;
+  const size_t nt = (size_t)ntx * nty;
+  sm_context* const ectx = ctx;         // errors are reported on the caller's handle
+  ctx = c;                              // CK writes ctx->err: the computing context's
+  auto done = [&](int r) { return ectx->group ? grp_err(ectx, 0, r) : r; };
+  CK(cudaSetDevice(c->cfg.device));
+  DevTmp t;
+  // about 37 B per cell: H, W, D, rcv, indeg, dir, area
+  double *H = nullptr, *W = nullptr;
+  int32_t *D = nullptr, *rcv = nullptr, *indeg = nullptr;
+  int8_t* dir8 = nullptr;
+  unsigned long long *A = nullptr, *cnt = nullptr;
+  unsigned int* act = nullptr;
+  if ((rc = snap_alloc(c, t, N * 8, (void**)&H)) != SM_OK || (rc = snap_alloc(c, t, N * 8, (void**)&W)) != SM_OK ||
+      (rc = snap_alloc(c, t, N * 4, (void**)&D)) != SM_OK || (rc = snap_alloc(c, t, nt * 8, (void**)&act)) != SM_OK ||
+      (rc = snap_alloc(c, t, DC_N * 8, (void**)&cnt)) != SM_OK)
+    return done(rc);
+  if (want_rcv && ((rc = snap_alloc(c, t, N * 4, (void**)&rcv)) != SM_OK ||
+                   (rc = snap_alloc(c, t, N * 4, (void**)&indeg)) != SM_OK || (rc = snap_alloc(c, t, N, (void**)&dir8)) != SM_OK))
+    return done(rc);
+  if (area && (rc = snap_alloc(c, t, N * 8, (void**)&A)) != SM_OK) return done(rc);
+  CK(cudaMemsetAsync(cnt, 0, DC_N * 8, c->stream));
+  DrainTimer tm;
+  tm.e.device = c->cfg.device;
+  CK(cudaEventCreate(&tm.e.e0));
+  CK(cudaEventCreate(&tm.e.e1));
+  const int G = c->num_sms * 8;
+  // the nl launches enqueued by f, timed as phase `ph`
+  auto timed = [&](int ph, int nl, auto f) -> int {
+    CK(cudaEventRecord(tm.e.e0, c->stream));
+    f();
+    c->launches += nl;
+    CK(cudaGetLastError());
+    CK(cudaEventRecord(tm.e.e1, c->stream));
+    CK(cudaEventSynchronize(tm.e.e1));
+    float ms = 0.f;
+    CK(cudaEventElapsedTime(&ms, tm.e.e0, tm.e.e1));
+    tm.ms[ph] += ms;
+    return SM_OK;
+  };
+  sm_drain_stats st = {};
+  const int ground = (flags & SM_DRAIN_GROUND) ? 1 : 0;
+  if ((rc = timed(0, 1, [&] {
+         if (multi) k_drain_heights<true><<<G, 256, 0, c->stream>>>(c->d, ground, H, W);
+         else k_drain_heights<false><<<G, 256, 0, c->stream>>>(c->d, ground, H, W);
+       })) != SM_OK)
+    return done(rc);
+  if ((rc = drain_relax<false>(c, tm, 1, H, W, nullptr, act, cnt + DC_MARKS, &st.fill_passes)) != SM_OK) return done(rc);
+  if ((rc = timed(2, 1, [&] { k_drain_classify<<<G, 256, 0, c->stream>>>(H, W, D, dimx, dimy, cnt); })) != SM_OK)
+    return done(rc);
+  if (want_rcv) {
+    if ((rc = drain_relax<true>(c, tm, 2, nullptr, W, D, act, cnt + DC_MARKS, &st.dist_passes)) != SM_OK) return done(rc);
+    CK(cudaMemsetAsync(indeg, 0, N * 4, c->stream));
+    if ((rc = timed(3, 2, [&] {
+           k_drain_receivers<<<G, 256, 0, c->stream>>>(W, D, dimx, dimy, dir8, rcv, indeg, A, cnt);
+           k_drain_outlets<<<G, 256, 0, c->stream>>>(indeg, dimx, dimy, cnt);
+         })) != SM_OK)
+      return done(rc);
+    if (area) {
+      CK(cudaMemcpyAsync(D, indeg, N * 4, cudaMemcpyDeviceToDevice, c->stream));     // D is free now: the walkers' rem
+      if ((rc = timed(4, 1, [&] { k_drain_area<<<G, 256, 0, c->stream>>>(rcv, indeg, D, A, N, cnt + DC_LONGEST); })) != SM_OK)
+        return done(rc);
+    }
+    if (basin) {      // indeg is free now: the jump pointers
+      if ((rc = timed(5, 1, [&] { k_drain_basin_init<<<G, 256, 0, c->stream>>>(rcv, indeg, N); })) != SM_OK) return done(rc);
+      for (;;) {
+        unsigned long long ch = 0;
+        CK(cudaMemsetAsync(cnt + DC_JUMP, 0, 8, c->stream));
+        if ((rc = timed(5, 1, [&] { k_drain_jump<<<G, 256, 0, c->stream>>>(indeg, N, cnt + DC_JUMP); })) != SM_OK) return done(rc);
+        CK(cudaMemcpy(&ch, cnt + DC_JUMP, 8, cudaMemcpyDeviceToHost));
+        st.jump_passes++;
+        if (!ch) break;
+      }
+    }
+  }
+  unsigned long long h_cnt[DC_N] = {};
+  CK(cudaMemcpy(h_cnt, cnt, sizeof(h_cnt), cudaMemcpyDeviceToHost));
+  if (h_cnt[DC_BAD]) return done(fail(c, SM_ERR_CUDA, "sm_drainage: a cell without a receiver after the fill (internal error)"));
+  // outputs: the cells [c0, c0 + m) of the whole-map rasters
+  const cudaMemcpyKind kind = cudaMemcpyDefault;
+  if (spill) CK(cudaMemcpyAsync(spill, W + c0, m * 8, kind, c->stream));
+  if (dir) CK(cudaMemcpyAsync(dir, dir8 + c0, m, kind, c->stream));
+  if (area) CK(cudaMemcpyAsync(area, A + c0, m * 8, kind, c->stream));
+  if (basin) {
+    int64_t* b64 = (int64_t*)H;      // H is free now
+    k_drain_basin_out<<<G, 256, 0, c->stream>>>(indeg, c0, m, b64);
+    c->launches++;
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(basin, b64, m * 8, kind, c->stream));
+  }
+  CK(cudaStreamSynchronize(c->stream));
+  if (ectx->group) ectx->group->dirty = false;
+  st.flat_cells = (int64_t)h_cnt[DC_FLAT];
+  st.depressed_cells = (int64_t)h_cnt[DC_DEPRESSED];
+  st.outlets = (int64_t)h_cnt[DC_OUTLETS];
+  st.longest_walk = (int64_t)h_cnt[DC_LONGEST];
+  for (int i = 0; i < 6; i++) {
+    st.phase_ms[i] = tm.ms[i];
+    st.device_ms += tm.ms[i];
+  }
   if (stats) *stats = st;
   return SM_OK;
 }

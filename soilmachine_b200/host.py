@@ -136,6 +136,13 @@ class Simulation:
         sm_voxelize): (nz, x1 - x0, y1 - y0) uint8, 255 where no section holds the height."""
         return self.ctx.voxelize(x0, x1, y0, y1, z0, dz, nz)
 
+    def drainage(self, ground=False):
+        """How the map drains (capi.Context.drainage, sm_drainage): a dict of (dimx, dimy) rasters - spill (the spill
+        height), dir (the receiver's neighbour index, -1 on the border), area (cells draining through each cell) and
+        basin (the border cell each cell drains to, as x*dimy + y).  ground=True reads the ground under standing water.
+        The call's stats are kept in self.ctx.drain_stats."""
+        return self.ctx.drainage(ground)
+
     def relax(self, max_passes, transferloop=0):
         """Relax the slopes of the whole map (capi.Context.relax, sm_relax): Particle::cascade at every cell, pass after
         pass in a fixed phase order, until a pass changes nothing or max_passes passes have run.  Returns the stats."""

@@ -171,6 +171,14 @@ class VirtualShards:
         self.view_stats = sum_view_stats([st for _, st in parts if st is not None])
         return np.concatenate([p for p, _ in parts], axis=1)
 
+    def drainage(self, ground=False):
+        """sm_drainage over the whole map: every rank computes the whole map and returns its strip, the strips are
+        joined along x.  Returns the dict of (dimx, dimy) rasters; rank 0's DrainStats are kept in self.drain_stats."""
+        self.sync()
+        parts = [c.drainage(ground) for c in self.ctx]
+        self.drain_stats = self.ctx[0].drain_stats
+        return {k: np.concatenate([p[k] for p in parts], axis=0) for k in parts[0]}
+
     def heights(self):
         return np.concatenate([c.heights() for c in self.ctx], axis=0)
 
@@ -340,6 +348,13 @@ class DistShard:
         have completed, so all ranks call it; the caller joins the strips along x."""
         self._settle()
         return self.ctx.composition(types, lo, hi, below_surface, pore_water)
+
+    def drainage(self, ground=False):
+        """sm_drainage on this rank: the rank computes the whole map through the peer pointers and returns its strip,
+        a dict of (x1 - x0, dimy) rasters (basin holds global indices).  Every rank's earlier work must have completed,
+        so all ranks call it; each repeats the whole-map work."""
+        self._settle()
+        return self.ctx.drainage(ground)
 
     def voxelize(self, x0, x1, y0, y1, z0, dz, nz):
         """sm_voxelize on this rank's part of the window (global coordinates), the window cut at the strip edges:
