@@ -385,11 +385,11 @@ template <class W, class A> SM_HD int water_move_coop(W& w, A& a, WaterP& p, Wat
     const float mx = n.x * (1.0f - f) + p.sx * f;
     const float my = n.z * (1.0f - f) + p.sy * f;
     const float inv = 1.0f / sqrtf(mx * mx + my * my);              // :61 sqrt(2)*normalize
-    p.sx = SM_SQRT2F * (mx * inv);
-    p.sy = SM_SQRT2F * (my * inv);
+    p.sx = host_nan(SM_SQRT2F * (mx * inv));                        // host_nan: sm_core.cuh
+    p.sy = host_nan(SM_SQRT2F * (my * inv));
   }
-  p.px += p.sx;                                                     // :62
-  p.py += p.sy;
+  p.px = host_nan(p.px + p.sx);                                     // :62
+  p.py = host_nan(p.py + p.sy);
   if (!(p.px >= 0.0f && p.py >= 0.0f) ||                            // :65-69
       !(p.px < (float)dimx - 1.0f && p.py < (float)dimy - 1.0f)) {
     if (A::kBudget && w.lead()) a.s->acc[3] += p.sediment * p.volume;

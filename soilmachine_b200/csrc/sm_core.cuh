@@ -368,6 +368,15 @@ template <int DEPTH, class A> struct Cascade {
 // ------------------------------------------------------------------------------------------------
 #define SM_SQRT2F 1.41421354f   // sqrt(2.0f) rounded to float (water.h:61)
 
+// A NaN with the bits the reference's x86 build gives it.  SSE returns the default NaN 0xFFC00000 for an invalid
+// operation and carries that NaN through the arithmetic after it; CUDA returns 0x7FFFFFFF for every NaN result.
+// water.h:60-62 makes one when mix(n.xz, speed, friction) is the zero vector (friction 1 on a particle at rest:
+// normalize is 0 * inf); the particle then leaves the map, but its speed and position stay in its state.
+SM_HD float host_nan(float v) {
+  union { uint32_t u; float f; } nan = {0xFFC00000u};
+  return v == v ? v : nan.f;
+}
+
 // ctor body water.h:14-17 / wind.h:17-20: what the particle transports
 template <class A> SM_HD uint32_t spawn_contains(A& a, float px, float py) {
   int ix = (int)roundf(px), iy = (int)roundf(py);
@@ -410,11 +419,11 @@ template <class A> SM_HD int water_move(A& a, WaterP& p, WaterMid& m) {
     float mx = n.x * (1.0f - f) + p.sx * f;
     float my = n.z * (1.0f - f) + p.sy * f;
     float inv = 1.0f / sqrtf(mx * mx + my * my);                    // :61 sqrt(2)*normalize
-    p.sx = SM_SQRT2F * (mx * inv);
-    p.sy = SM_SQRT2F * (my * inv);
+    p.sx = host_nan(SM_SQRT2F * (mx * inv));
+    p.sy = host_nan(SM_SQRT2F * (my * inv));
   }
-  p.px += p.sx;                                                     // :62
-  p.py += p.sy;
+  p.px = host_nan(p.px + p.sx);                                     // :62
+  p.py = host_nan(p.py + p.sy);
   if (!(p.px >= 0.0f && p.py >= 0.0f) ||                            // :65-69
       !(p.px < (float)dimx - 1.0f && p.py < (float)dimy - 1.0f)) {
     p.volume = 0.0;
